@@ -123,6 +123,18 @@ int lkb_ls_power_chi2(const double* t, const void* y, int y_dtype, const int64_t
                       const double* freq, const int64_t* freq_offsets, int64_t F, int nterms,
                       int normalization, const double* norm_scale, float* power, double* theta,
                       int mem, void* stream);
+/* The same with the kernel family chosen by the caller (lkb_ls_power_chi2 is LKB_LS_ALGO_SIMT):
+ *   LKB_LS_ALGO_SIMT   direct fp64 sums (ls_chi2_kernel);
+ *   LKB_LS_ALGO_NUFFT  the harmonic trig sums from the fp32 type-1 NUFFT of the flux and of unit strengths, fp64
+ *                      solve; needs one shared regular host-visible grid f_k = (k0 + k) df (integer k0), sorted
+ *                      times, df * baseline <= 1, >= 8 cadences per light curve and theta == NULL, else
+ *                      LKB_E_UNSUPPORTED;
+ *   LKB_LS_ALGO_AUTO   NUFFT when it qualifies and sum(N) * F >= 5e7 (DESIGN.md section 4, K1c), else SIMT.
+ * lkb_ls_last_algo reports which family ran. */
+int lkb_ls_power_chi2_ex(const double* t, const void* y, int y_dtype, const int64_t* offsets, int B,
+                         const double* freq, const int64_t* freq_offsets, int64_t F, int nterms,
+                         int normalization, const double* norm_scale, float* power, double* theta,
+                         int mem, void* stream, int algo);
 
 /* K2: batch sharing ONE cadence grid (BASELINE config 2); same math, but the
  * sin/cos design matrix is synthesised once per (frequency, cadence) tile and

@@ -42,6 +42,8 @@ SIGNATURES = {
                                 c_int]),
     "lkb_ls_power_chi2": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp,
                                   c_int, c_vp]),
+    "lkb_ls_power_chi2_ex": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp,
+                                     c_vp, c_int, c_vp, c_int]),
     "lkb_ls_power_shared": (c_int, [c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_int,
                                     c_vp, c_int]),
     "lkb_bls_power": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_vp, c_int, c_int, c_int,

@@ -211,7 +211,7 @@ int ls_power_ragged(const double*, const void*, int, const int64_t*, int, const 
 int ls_power_shared(const double*, const void*, int, int, int64_t, const double*, int64_t, int, const double*,
                     float*, int, cudaStream_t, int);
 int ls_power_chi2(const double*, const void*, int, const int64_t*, int, const double*, const int64_t*, int64_t, int,
-                  int, const double*, float*, double*, int, cudaStream_t);
+                  int, const double*, float*, double*, int, cudaStream_t, int);
 int bls_power(const double*, const double*, const double*, const int64_t*, int, const double*, int64_t,
               const double*, int, int, int, double*, double*, double*, double*, double*, double*, double*, int32_t*,
               int, cudaStream_t);
@@ -341,7 +341,15 @@ int lkb_ls_power_chi2(const double* t, const void* y, int y_dtype, const int64_t
                       float* power, double* theta, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return ls_power_chi2(t, y, y_dtype, offsets, B, freq, freq_offsets, F, nterms, normalization, norm_scale, power,
-                       theta, mem, (cudaStream_t)stream);
+                       theta, mem, (cudaStream_t)stream, LKB_LS_ALGO_SIMT);
+}
+
+int lkb_ls_power_chi2_ex(const double* t, const void* y, int y_dtype, const int64_t* offsets, int B, const double* freq,
+                         const int64_t* freq_offsets, int64_t F, int nterms, int normalization, const double* norm_scale,
+                         float* power, double* theta, int mem, void* stream, int algo) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return ls_power_chi2(t, y, y_dtype, offsets, B, freq, freq_offsets, F, nterms, normalization, norm_scale, power,
+                       theta, mem, (cudaStream_t)stream, algo);
 }
 
 int lkb_bls_power(const double* t, const double* y, const double* dy, const int64_t* offsets, int B,

@@ -30,6 +30,26 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
                            const int64_t* h_off, int B, int64_t ptotal, int64_t nmax, const double* d_span,
                            const double* h_span, const double* d_ysum, int64_t F, double f0, double df,
                            int normalization, const double* d_ns, float* d_pow, cudaStream_t st);
+int ls_nufft_chi2_ragged_launch(const double* d_t, const float* d_y, const int64_t* d_off, const int64_t* d_po,
+                                const int64_t* h_off, int B, int64_t ptotal, int64_t nmax, const double* d_span,
+                                const double* h_span, const double* d_ysum, int64_t F, double f0, double df,
+                                int normalization, const double* d_ns, float* d_pow, cudaStream_t st, int nterms);
+
+// `auto` of the multi-term periodogram takes the NUFFT path from this much work on (sum over the light curves of
+// cadences x frequency bins).  Measured crossover on an H100 (tools/bench_chi2.py, DESIGN.md section 4 K1c): at 2e7 the
+// direct kernel is faster for nterms 1-3 and as fast at 4; at 8e7 the NUFFT path is faster for every nterms.
+constexpr double LS_CHI2_NUFFT_MIN_WORK = 5e7;
+
+// Is fq[0 .. Fb) the regular grid f0 + k df (f0 >= 0, df > 0, every bin within 1e-6 df)?
+static bool regular_grid(const double* fq, int64_t Fb, double* f0, double* df) {
+  if (Fb < 2 || Fb >= ((int64_t)1 << 31)) return false;
+  *f0 = fq[0];
+  *df = fq[1] - fq[0];
+  if (!(*f0 >= 0.0) || !(*df > 0.0)) return false;
+  for (int64_t k = 0; k < Fb; ++k)
+    if (fabs(fq[k] - (*f0 + (double)k * *df)) > 1e-6 * *df) return false;
+  return true;
+}
 
 // Per-cadence entry of a regular-grid light curve (ragged path): fixed-point phases of the grid origin and of one
 // grid step, plus the fp32 rotation by one step - the bins after a warp's first are obtained by rotating (cos, sin)
@@ -508,74 +528,6 @@ ls_shared_simt_kernel(const double* __restrict__ t, int64_t N, int64_t Npad, con
 // Optionally returns the fitted parameters theta (LombScargle.model, periodogram.py:1010).
 // =====================================================================================
 template <int NT>
-struct Chi2Sums {
-  double S[2 * NT], C[2 * NT], YS[NT], YC[NT];
-  __device__ __forceinline__ void zero() {
-#pragma unroll
-    for (int j = 0; j < 2 * NT; ++j) { S[j] = 0.0; C[j] = 0.0; }
-#pragma unroll
-    for (int j = 0; j < NT; ++j) { YS[j] = 0.0; YC[j] = 0.0; }
-  }
-};
-
-template <int NT>
-__device__ void chi2_solve(const Chi2Sums<NT>& d, double N, double ysum, double& power, double* theta) {
-  constexpr int M = 2 * NT + 1;
-  double A[M][M + 1];
-  auto Cd = [&](int m) { return m == 0 ? N : d.C[m - 1]; };
-  auto Sd = [&](int m) { return m == 0 ? 0.0 : (m > 0 ? d.S[m - 1] : -d.S[-m - 1]); };
-  A[0][0] = N;
-  A[0][M] = ysum;
-  for (int i = 1; i <= NT; ++i) {
-    const int si = 2 * i - 1, ci = 2 * i;
-    A[0][si] = A[si][0] = d.S[i - 1];
-    A[0][ci] = A[ci][0] = d.C[i - 1];
-    A[si][M] = d.YS[i - 1];
-    A[ci][M] = d.YC[i - 1];
-    for (int j = 1; j <= NT; ++j) {
-      const int sj = 2 * j - 1, cj = 2 * j;
-      const int dm = i > j ? i - j : j - i;
-      A[si][sj] = 0.5 * (Cd(dm) - Cd(i + j));
-      A[ci][cj] = 0.5 * (Cd(dm) + Cd(i + j));
-      A[si][cj] = 0.5 * (Sd(i + j) + Sd(i - j));
-      A[cj][si] = A[si][cj];
-    }
-  }
-  double rhs[M];
-  for (int i = 0; i < M; ++i) rhs[i] = A[i][M];
-  bool ok = true;
-  for (int c = 0; c < M && ok; ++c) {
-    int piv = c;
-    for (int r = c + 1; r < M; ++r)
-      if (fabs(A[r][c]) > fabs(A[piv][c])) piv = r;
-    if (!(fabs(A[piv][c]) > 0.0)) { ok = false; break; }
-    if (piv != c)
-      for (int k = 0; k <= M; ++k) { const double tmp = A[c][k]; A[c][k] = A[piv][k]; A[piv][k] = tmp; }
-    for (int r = c + 1; r < M; ++r) {
-      const double fct = A[r][c] / A[c][c];
-      for (int k = c; k <= M; ++k) A[r][k] -= fct * A[c][k];
-    }
-  }
-  double th[M];
-  const double qnan = __longlong_as_double(0x7ff8000000000000ll);
-  if (ok) {
-    for (int c = M - 1; c >= 0; --c) {
-      double v = A[c][M];
-      for (int k = c + 1; k < M; ++k) v -= A[c][k] * th[k];
-      th[c] = v / A[c][c];
-    }
-    double acc = 0.0;
-    for (int i = 0; i < M; ++i) acc += rhs[i] * th[i];
-    power = 0.5 * acc;
-  } else {
-    power = qnan;
-    for (int i = 0; i < M; ++i) th[i] = qnan;
-  }
-  if (theta)
-    for (int i = 0; i < M; ++i) theta[i] = th[i];
-}
-
-template <int NT>
 __global__ void __launch_bounds__(LS_WARPS * 32)
 ls_chi2_kernel(const double* __restrict__ tws, const double* __restrict__ yws, const int64_t* __restrict__ offsets,
                const int64_t* __restrict__ poffsets, const double* __restrict__ freq,
@@ -635,26 +587,11 @@ ls_chi2_kernel(const double* __restrict__ tws, const double* __restrict__ yws, c
     // fp64 throughout: this path is not the throughput path, and the normal equations of a
     // multi-harmonic fit are far less forgiving than the single-term closed form
     for (int i = lane; i < cnt; i += 32) {
-      const double yy = s_y[buf][i];
-      double s1, c1;
-      ls_sincos_cycles_f64(fr * s_t[buf][i], s1, c1);
-      double sj = s1, cj = c1;
-#pragma unroll
-      for (int j = 0; j < 2 * NT; ++j) {
-        d.S[j] += sj;
-        d.C[j] += cj;
-        if (j < NT) { d.YS[j] = fma(yy, sj, d.YS[j]); d.YC[j] = fma(yy, cj, d.YC[j]); }
-        const double sn = fma(sj, c1, cj * s1), cn = fma(cj, c1, -sj * s1);
-        sj = sn;
-        cj = cn;
-      }
+      chi2_add<NT>(d, s_y[buf][i], fr * s_t[buf][i]);
     }
     __syncthreads();
   }
-#pragma unroll
-  for (int j = 0; j < 2 * NT; ++j) { d.S[j] = warp_sum(d.S[j]); d.C[j] = warp_sum(d.C[j]); }
-#pragma unroll
-  for (int j = 0; j < NT; ++j) { d.YS[j] = warp_sum(d.YS[j]); d.YC[j] = warp_sum(d.YC[j]); }
+  chi2_warp_reduce<NT>(d);
   if (lane == 0 && f_ok) {
     double p;
     chi2_solve<NT>(d, (double)n, ysum[b], p, theta_out ? theta_out + (po_out + fi) * (2 * NT + 1) : nullptr);
@@ -723,16 +660,9 @@ int ls_power_ragged(const double* t, const void* y, int y_dtype, const int64_t* 
     for (int b = 0; b < B && regular; ++b) {
       const int64_t fo = h_freq_offsets ? h_freq_offsets[b] : 0;
       const int64_t Fb = h_freq_offsets ? h_freq_offsets[b + 1] - fo : F;
-      const double* fq = freq_h + fo;
-      if (Fb < 2 || Fb >= ((int64_t)1 << 31)) { regular = false; break; }
-      const double f0 = fq[0], df = fq[1] - fq[0];
-      if (!(f0 >= 0.0) || !(df > 0.0)) { regular = false; break; }
-      for (int64_t k = 0; k < Fb; ++k)
-        if (fabs(fq[k] - (f0 + (double)k * df)) > 1e-6 * df) { regular = false; break; }
-      h_f0[b] = f0;
-      h_df[b] = df;
-      if (!h_freq_offsets) {          // one shared grid: same (f0, df) for every light curve
-        for (int bb = 1; bb < B; ++bb) { h_f0[bb] = f0; h_df[bb] = df; }
+      regular = regular_grid(freq_h + fo, Fb, &h_f0[b], &h_df[b]);
+      if (regular && !h_freq_offsets) {          // one shared grid: same (f0, df) for every light curve
+        for (int bb = 1; bb < B; ++bb) { h_f0[bb] = h_f0[0]; h_df[bb] = h_df[0]; }
         break;
       }
     }
@@ -832,8 +762,10 @@ int ls_power_ragged(const double* t, const void* y, int y_dtype, const int64_t* 
 
 int ls_power_chi2(const double* t, const void* y, int y_dtype, const int64_t* h_offsets, int B, const double* freq,
                   const int64_t* h_freq_offsets, int64_t F, int nterms, int normalization, const double* norm_scale,
-                  float* power, double* theta, int mem, cudaStream_t st) {
+                  float* power, double* theta, int mem, cudaStream_t st, int algo) {
   LKB_REQUIRE(B > 0 && B <= 65535 && t && y && h_offsets && freq && power, "lkb_ls_power_chi2: null/bad argument");
+  LKB_REQUIRE(algo == LKB_LS_ALGO_AUTO || algo == LKB_LS_ALGO_SIMT || algo == LKB_LS_ALGO_NUFFT,
+              "lkb_ls_power_chi2: algo must be AUTO, SIMT (direct sums) or NUFFT");
   LKB_REQUIRE(y_dtype == LKB_DTYPE_F32 || y_dtype == LKB_DTYPE_F64, "lkb_ls_power_chi2: bad y_dtype");
   LKB_REQUIRE(nterms >= 1 && nterms <= 4, "lkb_ls_power_chi2: nterms must be in [1, 4]");
   LKB_REQUIRE(normalization >= 0 && normalization <= 2, "lkb_ls_power_chi2: bad normalization");
@@ -885,6 +817,62 @@ int ls_power_chi2(const double* t, const void* y, int y_dtype, const int64_t* h_
   double* d_theta = nullptr;
   LKB_TRY(stage_out_alloc<float>(mem, WS_OUT0, power, out_count, &d_pow));
   LKB_TRY(stage_out_alloc<double>(mem, WS_OUT1, theta, out_count * M, &d_theta));
+
+  // NUFFT path of ls_nufft.cu (one shared regular grid f_k = (k0 + k) df, no theta): what `auto` picks when the job is
+  // large enough to pay for its transforms; light curves that do not qualify (fewer than 8 cadences, unsorted times,
+  // df * baseline > 1, fine grids outside the v2 range) send the whole call to the direct kernel under `auto` and fail
+  // an explicit NUFFT request.  LKB_LS_RAGGED_NUFFT=0 keeps `auto` on the direct kernel.
+  if (algo == LKB_LS_ALGO_NUFFT ||
+      (algo == LKB_LS_ALGO_AUTO && ls_nufft_ragged_enabled() && (double)total * (double)F >= LS_CHI2_NUFFT_MIN_WORK)) {
+    int64_t nmax = 0, nmin = INT64_MAX;
+    for (int b = 0; b < B; ++b) {
+      const int64_t n = h_offsets[b + 1] - h_offsets[b];
+      nmax = n > nmax ? n : nmax;
+      nmin = n < nmin ? n : nmin;
+    }
+    double f0 = 0.0, df = 0.0;
+    bool eligible = !h_freq_offsets && !theta && nmin >= 8;
+    if (eligible) {
+      std::vector<double> h_freq_copy;
+      const double* freq_h = freq;
+      if (mem == LKB_MEM_DEVICE) {
+        h_freq_copy.resize((size_t)F);
+        LKB_CUDA_CHECK(cudaMemcpyAsync(h_freq_copy.data(), freq, sizeof(double) * (size_t)F, cudaMemcpyDeviceToHost, st));
+        LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+        freq_h = h_freq_copy.data();
+      }
+      eligible = regular_grid(freq_h, F, &f0, &df);
+    }
+    int rc = LKB_E_UNSUPPORTED;
+    if (eligible) {
+      // the transforms take the centred flux in fp32, as in ls_power_ragged (ysum: sum of the fp32 values)
+      float* d_yf = nullptr;
+      LKB_TRY(ws_get_t<float>(WS_E, ptotal + 4, &d_yf));
+      if (y_dtype == LKB_DTYPE_F32)
+        ls_prep_ragged_kernel<float><<<B, 256, 0, st>>>(dt_in, (const float*)dy_in, d_off, d_po, d_t, d_yf, d_span,
+                                                        nullptr, nullptr, nullptr, d_ysum);
+      else
+        ls_prep_ragged_kernel<double><<<B, 256, 0, st>>>(dt_in, (const double*)dy_in, d_off, d_po, d_t, d_yf, d_span,
+                                                         nullptr, nullptr, nullptr, d_ysum);
+      LKB_LAUNCH_CHECK();
+      std::vector<double> h_span(B);
+      LKB_CUDA_CHECK(cudaMemcpyAsync(h_span.data(), d_span, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+      LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+      rc = ls_nufft_chi2_ragged_launch(d_t, d_yf, d_off, d_po, h_offsets, B, ptotal, nmax, d_span, h_span.data(), d_ysum,
+                                       F, f0, df, normalization, d_ns, d_pow, st, nterms);
+      if (rc == LKB_OK) {
+        g_last_ls_algo = LKB_LS_ALGO_NUFFT;
+        LKB_TRY(stage_out_copy<float>(mem, power, d_pow, out_count, st));
+        if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+        return LKB_OK;
+      }
+    } else {
+      set_error("lkb_ls_power_chi2: the NUFFT path needs one host-visible, regular, shared frequency grid, no theta "
+                "and at least 8 cadences per light curve");
+    }
+    if (rc != LKB_E_UNSUPPORTED || algo == LKB_LS_ALGO_NUFFT) return rc;
+  }
+  g_last_ls_algo = LKB_LS_ALGO_SIMT;
   if (y_dtype == LKB_DTYPE_F32)
     ls_prep_ragged_kernel<float><<<B, 256, 0, st>>>(dt_in, (const float*)dy_in, d_off, d_po, d_t, nullptr, d_span,
                                                     nullptr, nullptr, nullptr, d_ysum, d_y);

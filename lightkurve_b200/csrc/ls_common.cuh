@@ -170,4 +170,100 @@ __device__ __forceinline__ float ls_epilogue_shared(float ch, float sh, const fl
   return p;
 }
 
+// Multi-term ("chi2") periodogram, shared by the direct kernel (ls.cu: ls_chi2_kernel) and the NUFFT path's low rows
+// (ls_nufft.cu): the harmonic trig sums S_j, C_j (j <= 2n) and YS_j, YC_j (j <= n) of one frequency, and the fp64
+// solve of the (2n+1)x(2n+1) normal equations they give.
+template <int NT>
+struct Chi2Sums {
+  double S[2 * NT], C[2 * NT], YS[NT], YC[NT];
+  __device__ __forceinline__ void zero() {
+#pragma unroll
+    for (int j = 0; j < 2 * NT; ++j) { S[j] = 0.0; C[j] = 0.0; }
+#pragma unroll
+    for (int j = 0; j < NT; ++j) { YS[j] = 0.0; YC[j] = 0.0; }
+  }
+};
+
+template <int NT>
+__device__ void chi2_solve(const Chi2Sums<NT>& d, double N, double ysum, double& power, double* theta) {
+  constexpr int M = 2 * NT + 1;
+  double A[M][M + 1];
+  auto Cd = [&](int m) { return m == 0 ? N : d.C[m - 1]; };
+  auto Sd = [&](int m) { return m == 0 ? 0.0 : (m > 0 ? d.S[m - 1] : -d.S[-m - 1]); };
+  A[0][0] = N;
+  A[0][M] = ysum;
+  for (int i = 1; i <= NT; ++i) {
+    const int si = 2 * i - 1, ci = 2 * i;
+    A[0][si] = A[si][0] = d.S[i - 1];
+    A[0][ci] = A[ci][0] = d.C[i - 1];
+    A[si][M] = d.YS[i - 1];
+    A[ci][M] = d.YC[i - 1];
+    for (int j = 1; j <= NT; ++j) {
+      const int sj = 2 * j - 1, cj = 2 * j;
+      const int dm = i > j ? i - j : j - i;
+      A[si][sj] = 0.5 * (Cd(dm) - Cd(i + j));
+      A[ci][cj] = 0.5 * (Cd(dm) + Cd(i + j));
+      A[si][cj] = 0.5 * (Sd(i + j) + Sd(i - j));
+      A[cj][si] = A[si][cj];
+    }
+  }
+  double rhs[M];
+  for (int i = 0; i < M; ++i) rhs[i] = A[i][M];
+  bool ok = true;
+  for (int c = 0; c < M && ok; ++c) {
+    int piv = c;
+    for (int r = c + 1; r < M; ++r)
+      if (fabs(A[r][c]) > fabs(A[piv][c])) piv = r;
+    if (!(fabs(A[piv][c]) > 0.0)) { ok = false; break; }
+    if (piv != c)
+      for (int k = 0; k <= M; ++k) { const double tmp = A[c][k]; A[c][k] = A[piv][k]; A[piv][k] = tmp; }
+    for (int r = c + 1; r < M; ++r) {
+      const double fct = A[r][c] / A[c][c];
+      for (int k = c; k <= M; ++k) A[r][k] -= fct * A[c][k];
+    }
+  }
+  double th[M];
+  const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+  if (ok) {
+    for (int c = M - 1; c >= 0; --c) {
+      double v = A[c][M];
+      for (int k = c + 1; k < M; ++k) v -= A[c][k] * th[k];
+      th[c] = v / A[c][c];
+    }
+    double acc = 0.0;
+    for (int i = 0; i < M; ++i) acc += rhs[i] * th[i];
+    power = 0.5 * acc;
+  } else {
+    power = qnan;
+    for (int i = 0; i < M; ++i) th[i] = qnan;
+  }
+  if (theta)
+    for (int i = 0; i < M; ++i) theta[i] = th[i];
+}
+
+template <int NT>
+__device__ __forceinline__ void chi2_warp_reduce(Chi2Sums<NT>& d) {
+#pragma unroll
+  for (int j = 0; j < 2 * NT; ++j) { d.S[j] = warp_sum(d.S[j]); d.C[j] = warp_sum(d.C[j]); }
+#pragma unroll
+  for (int j = 0; j < NT; ++j) { d.YS[j] = warp_sum(d.YS[j]); d.YC[j] = warp_sum(d.YC[j]); }
+}
+
+// one cadence of the sums: flux yy at phase `phase` (cycles); harmonics from the angle-addition recurrence
+template <int NT>
+__device__ __forceinline__ void chi2_add(Chi2Sums<NT>& d, double yy, double phase) {
+  double s1, c1;
+  ls_sincos_cycles_f64(phase, s1, c1);
+  double sj = s1, cj = c1;
+#pragma unroll
+  for (int j = 0; j < 2 * NT; ++j) {
+    d.S[j] += sj;
+    d.C[j] += cj;
+    if (j < NT) { d.YS[j] = fma(yy, sj, d.YS[j]); d.YC[j] = fma(yy, cj, d.YC[j]); }
+    const double sn = fma(sj, c1, cj * s1), cn = fma(cj, c1, -sj * s1);
+    sj = sn;
+    cj = cn;
+  }
+}
+
 }  // namespace lkb

@@ -1211,16 +1211,100 @@ nufft_lowrows_ragged_kernel(const double* __restrict__ t, const float* __restric
                                     norm_scale ? norm_scale[b] : 1.0);
 }
 
+// Multi-term periodogram (nterms = NT), power[b, k] for the rows that are not "low" for light curve b.  Harmonic j of
+// f_k = (k0 + k) df is mode j kk of the same transforms: modes j kk (j <= NT) of the flux transform Zn [B][M / 2] give
+// YC_j, YS_j, modes j kk (j <= 2 NT) of the unit-strength transform Zwn [B][M2 / 2] give C_j, S_j.  dec / dec2 hold the
+// deconvolution factor of every mode index [0, NT (k0 + F)) / [0, 2 NT (k0 + F)).
+// A bin where some harmonic's window sum is nearly coherent, |C_j + i S_j| >= LS_CHI2_COHERENT N, is a low row in
+// disguise: j f sits near a multiple of the sampling rate of a near-regular cadence (a TESS 2-min light curve: 720 / d,
+// which the harmonics of a grid up to the Nyquist frequency reach), the normal matrix cancels like that of
+// f * baseline <= 2, and the fp32 sums miss the tolerance there (emulated 2-min light curves: up to 300x within one bin
+// of 720 / d).  Such bins take the direct fp64 sums, in this thread; irregular cadences never get near the limit.
+constexpr double LS_CHI2_COHERENT = 0.25;
+template <int NT>
+__global__ void __launch_bounds__(256)
+nufft2_finish_chi2_ragged_kernel(const float2* __restrict__ Zn, int p, const float2* __restrict__ Zwn, int p2,
+                                 const float2* __restrict__ dec, const float2* __restrict__ dec2, int64_t k0, int64_t F,
+                                 double f0, double df, const int64_t* __restrict__ off, const int64_t* __restrict__ poff,
+                                 const double* __restrict__ t, const float* __restrict__ y,
+                                 const double* __restrict__ span, const double* __restrict__ ysum, int normalization,
+                                 const double* __restrict__ norm_scale, int B, float* __restrict__ power) {
+  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid >= F * B) return;
+  const int64_t b = gid / F, k = gid - b * F;
+  const double fr = f0 + (double)k * df;
+  if (!(fr * span[b] > LS_LOWF_CYCLES)) return;
+  const int64_t M = (int64_t)1 << p, M2 = (int64_t)1 << p2, kk = k0 + k;
+  const float2* zw = Zwn + b * (M2 >> 1);
+  const float2* zy = Zn + b * (M >> 1);
+  Chi2Sums<NT> d;
+#pragma unroll
+  for (int j = 0; j < 2 * NT; ++j) {
+    const int64_t m = (j + 1) * kk;
+    const float2 a = nufft::cmul(v2_unpack_real(zw, m, M2), dec2[m]);
+    d.C[j] = (double)a.x;
+    d.S[j] = (double)a.y;
+  }
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+    const int64_t m = (j + 1) * kk;
+    const float2 h = nufft::cmul(v2_unpack_real(zy, m, M), dec[m]);
+    d.YC[j] = (double)h.x;
+    d.YS[j] = (double)h.y;
+  }
+  const int64_t n = off[b + 1] - off[b];
+  const double Nd = (double)n;
+  bool coherent = false;
+#pragma unroll
+  for (int j = 0; j < 2 * NT; ++j) coherent |= d.C[j] * d.C[j] + d.S[j] * d.S[j] >= LS_CHI2_COHERENT * LS_CHI2_COHERENT * Nd * Nd;
+  if (coherent) {
+    d.zero();
+    for (int64_t i = 0; i < n; ++i) chi2_add<NT>(d, (double)y[poff[b] + i], fr * t[poff[b] + i]);
+  }
+  double pw;
+  chi2_solve<NT>(d, Nd, ysum[b], pw, nullptr);
+  power[b * F + k] = ls_normalize(pw, Nd, normalization, norm_scale ? norm_scale[b] : 1.0);
+}
+
+// the rows with f * baseline_b <= LS_LOWF_CYCLES of the multi-term periodogram: direct fp64 sums (the accumulation of
+// ls.cu's ls_chi2_kernel), one warp per (row, light curve)
+template <int NT>
+__global__ void __launch_bounds__(128)
+nufft_lowrows_chi2_ragged_kernel(const double* __restrict__ t, const float* __restrict__ y,
+                                 const int64_t* __restrict__ off, const int64_t* __restrict__ poff,
+                                 const double* __restrict__ span, const double* __restrict__ ysum, double f0, double df,
+                                 int64_t F_low_max, int64_t F, int normalization, const double* __restrict__ norm_scale,
+                                 int B, float* __restrict__ power) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t job = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+  if (job >= F_low_max * B) return;
+  const int64_t b = job / F_low_max, k = job - b * F_low_max;
+  const double fr = f0 + (double)k * df;
+  if (k >= F || fr * span[b] > LS_LOWF_CYCLES) return;
+  const int64_t n = off[b + 1] - off[b], po = poff[b];
+  if (n <= 0) return;
+  Chi2Sums<NT> d;
+  d.zero();
+  for (int64_t i = lane; i < n; i += 32) chi2_add<NT>(d, (double)y[po + i], fr * t[po + i]);
+  chi2_warp_reduce<NT>(d);
+  if (lane == 0) {
+    double pw;
+    chi2_solve<NT>(d, (double)n, ysum[b], pw, nullptr);
+    power[b * F + k] = ls_normalize(pw, (double)n, normalization, norm_scale ? norm_scale[b] : 1.0);
+  }
+}
+
 }  // namespace
 
 namespace {
 // Ragged batch through the v2 transform: every light curve is one real series on the flux grid (2^p cells) and one on
 // the window grid (2^p2 cells, unit strengths); groups of light curves share the buffers when the fine grids of the
-// whole batch exceed cap_mb.
+// whole batch exceed cap_mb.  nterms = 0: the single-term periodogram (window modes kk, 2 kk; flux mode kk);
+// nterms = n in [1, 4]: the multi-term one (window modes j kk, j <= 2n; flux modes j kk, j <= n).
 int ls_nufft_ragged_v2(const double* d_t, const float* d_y, const int64_t* d_off, const int64_t* d_po, int B,
                        int64_t ptotal, int64_t nmax, const double* d_span, const double* h_span, const double* d_ysum,
                        int64_t F, double f0, double df, int64_t k0, int p, int p2, int w, float beta, double cap_mb,
-                       int normalization, const double* d_ns, float* d_pow, cudaStream_t st) {
+                       int normalization, const double* d_ns, float* d_pow, cudaStream_t st, int nterms) {
   const int64_t M = (int64_t)1 << p, M2 = (int64_t)1 << p2, Mh = M >> 1, Mh2 = M2 >> 1;
   double span_max = 0.0;
   for (int b = 0; b < B; ++b) span_max = fmax(span_max, h_span[b]);
@@ -1245,8 +1329,12 @@ int ls_nufft_ragged_v2(const double* d_t, const float* d_y, const int64_t* d_off
   LKB_TRY(ws_get_t<float2>(WS_P, (size_t)group * Mh2, &Tw));
   LKB_TRY(ws_get_t<float2>(WS_OUT3, (size_t)group * Mh2, &Zwn));
   LKB_TRY(ws_get_t<float2>(WS_OUT2, (size_t)group * std::max(cells, cells2), &G));
-  LKB_TRY(ws_get_t<float2>(WS_IN4, F, &dec));
-  LKB_TRY(ws_get_t<float2>(WS_IN5, 2 * (k0 + F), &dec2));
+  // flux modes below kmax, window modes below 2 kmax; the single-term finish indexes dec by row k, the multi-term one
+  // by mode index
+  const int64_t kmax = (int64_t)std::max(nterms, 1) * (k0 + F);
+  const int64_t dec_first = nterms ? 0 : k0, dec_len = nterms ? kmax : F;
+  LKB_TRY(ws_get_t<float2>(WS_IN4, dec_len, &dec));
+  LKB_TRY(ws_get_t<float2>(WS_IN5, 2 * kmax, &dec2));
   LKB_TRY(ws_get_t<int>(WS_IN6, 1, &flag));
 
   LKB_CUDA_CHECK(cudaMemsetAsync(flag, 0, sizeof(int), st));
@@ -1260,15 +1348,15 @@ int ls_nufft_ragged_v2(const double* d_t, const float* d_y, const int64_t* d_off
   LKB_CUDA_CHECK(cudaMemcpyAsync(&h_flag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   LKB_CUDA_CHECK(cudaStreamSynchronize(st));
   if (h_flag) { set_error("NUFFT (ragged): a light curve has unsorted times"); return LKB_E_UNSUPPORTED; }
-  LKB_LAUNCH(blocks_for(F, 128), 128, st, nufft_deconv_kernel)(k0, F, M, w, (double)beta, gl, dec);
+  LKB_LAUNCH(blocks_for(dec_len, 128), 128, st, nufft_deconv_kernel)(dec_first, dec_len, M, w, (double)beta, gl, dec);
   LKB_LAUNCH_CHECK();
-  LKB_LAUNCH(blocks_for(2 * (k0 + F), 128), 128, st, nufft_deconv_kernel)(0, 2 * (k0 + F), M2, w, (double)beta, gl, dec2);
+  LKB_LAUNCH(blocks_for(2 * kmax, 128), 128, st, nufft_deconv_kernel)(0, 2 * kmax, M2, w, (double)beta, gl, dec2);
   LKB_LAUNCH_CHECK();
 
   // kernel weights in FP64 from the time stamps (default; LKB_NUFFT_RAGGED_W32=1: the fp32 form, for A/B timing)
   const double* t_acc = getenv("LKB_NUFFT_RAGGED_W32") ? nullptr : d_t;
   const int ptc = V2_LOG_TILE - (p - 1 - V2_PB), ptc2 = V2_LOG_TILE - (p2 - 1 - V2_PB);
-  const int nk2 = (int)((k0 + F) >> (p - 1 - V2_PB)) + 1, nk2w = (int)((2 * (k0 + F)) >> (p2 - 1 - V2_PB)) + 1;
+  const int nk2 = (int)(kmax >> (p - 1 - V2_PB)) + 1, nk2w = (int)((2 * kmax) >> (p2 - 1 - V2_PB)) + 1;
   prof_begin(st);
   for (int b0 = 0; b0 < B; b0 += group) {
     const int Bg = std::min(group, B - b0);
@@ -1288,19 +1376,68 @@ int ls_nufft_ragged_v2(const double* d_t, const float* d_y, const int64_t* d_off
     LKB_LAUNCH_CHECK();
     LKB_TRY(v2_cols(G, T, p, n1max, Bg, tb, st));
     LKB_TRY(v2_rows(T, p, Bg, tb, nullptr, Zn, nk2, st));
-    LKB_LAUNCH(blocks_for(F * Bg, 256), 256, st, nufft2_finish_ragged_kernel)(
-        Zn, p, Zwn, p2, dec, dec2, k0, F, f0, df, off_g, d_span + b0, d_ysum + b0, normalization,
-        d_ns ? d_ns + b0 : nullptr, Bg, d_pow + (size_t)b0 * F);
+    const double* ns_g = d_ns ? d_ns + b0 : nullptr;
+    float* pow_g = d_pow + (size_t)b0 * F;
+#define LKB_CHI2_FINISH(NT)                                                                                            \
+  LKB_LAUNCH(blocks_for(F * Bg, 256), 256, st, nufft2_finish_chi2_ragged_kernel<NT>)(                                  \
+      Zn, p, Zwn, p2, dec, dec2, k0, F, f0, df, off_g, po_g, d_t, d_y, d_span + b0, d_ysum + b0, normalization, ns_g, \
+      Bg, pow_g)
+#define LKB_CHI2_LOW(NT)                                                                                               \
+  LKB_LAUNCH(blocks_for(F_low_max * Bg, 4), 128, st, nufft_lowrows_chi2_ragged_kernel<NT>)(                            \
+      d_t, d_y, off_g, po_g, d_span + b0, d_ysum + b0, f0, df, F_low_max, F, normalization, ns_g, Bg, pow_g)
+    switch (nterms) {
+      case 0:
+        LKB_LAUNCH(blocks_for(F * Bg, 256), 256, st, nufft2_finish_ragged_kernel)(
+            Zn, p, Zwn, p2, dec, dec2, k0, F, f0, df, off_g, d_span + b0, d_ysum + b0, normalization, ns_g, Bg, pow_g);
+        break;
+      case 1: LKB_CHI2_FINISH(1); break;
+      case 2: LKB_CHI2_FINISH(2); break;
+      case 3: LKB_CHI2_FINISH(3); break;
+      default: LKB_CHI2_FINISH(4); break;
+    }
     LKB_LAUNCH_CHECK();
     if (F_low_max > 0) {
-      LKB_LAUNCH(blocks_for(F_low_max * Bg, 4), 128, st, nufft_lowrows_ragged_kernel)(
-          d_t, d_y, off_g, po_g, d_span + b0, d_ysum + b0, f0, df, F_low_max, F, normalization,
-          d_ns ? d_ns + b0 : nullptr, Bg, d_pow + (size_t)b0 * F);
+      switch (nterms) {
+        case 0:
+          LKB_LAUNCH(blocks_for(F_low_max * Bg, 4), 128, st, nufft_lowrows_ragged_kernel)(
+              d_t, d_y, off_g, po_g, d_span + b0, d_ysum + b0, f0, df, F_low_max, F, normalization, ns_g, Bg, pow_g);
+          break;
+        case 1: LKB_CHI2_LOW(1); break;
+        case 2: LKB_CHI2_LOW(2); break;
+        case 3: LKB_CHI2_LOW(3); break;
+        default: LKB_CHI2_LOW(4); break;
+      }
       LKB_LAUNCH_CHECK();
     }
+#undef LKB_CHI2_FINISH
+#undef LKB_CHI2_LOW
   }
   prof_end(st);
   return LKB_OK;
+}
+
+// f_k = (k0 + k) df with integer k0, and 0 < df * baseline <= 1 for every light curve
+int ragged_grid_check(int B, const double* h_span, double f0, double df, int64_t* k0) {
+  const double q = f0 / df, k0d = rint(q);
+  if (!(df > 0.0) || !(f0 >= 0.0) || fabs(q - k0d) > 1e-9 * fmax(1.0, q) || k0d > 1.0e7) {
+    set_error("NUFFT (ragged): the grid is not f_k = (k0 + k) df with integer k0");
+    return LKB_E_UNSUPPORTED;
+  }
+  for (int b = 0; b < B; ++b) {
+    if (!(h_span[b] > 0.0) || !(df * h_span[b] <= 1.0 + 1e-9)) {
+      set_error("NUFFT (ragged): a light curve has zero baseline or df * baseline > 1");
+      return LKB_E_UNSUPPORTED;
+    }
+  }
+  *k0 = (int64_t)k0d;
+  return LKB_OK;
+}
+
+// fine-grid budget of a ragged call: LKB_NUFFT_RAGGED_MB (default 16384)
+double ragged_cap_mb() {
+  double cap_mb = 16384.0;
+  if (const char* e = getenv("LKB_NUFFT_RAGGED_MB")) { const double v = atof(e); if (v > 0.0) cap_mb = v; }
+  return cap_mb;
 }
 }  // namespace
 
@@ -1320,27 +1457,16 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
                            const double* h_span, const double* d_ysum, int64_t F, double f0, double df,
                            int normalization, const double* d_ns, float* d_pow, cudaStream_t st) {
   (void)h_off;
-  const double q = f0 / df, k0d = rint(q);
-  if (!(df > 0.0) || !(f0 >= 0.0) || fabs(q - k0d) > 1e-9 * fmax(1.0, q) || k0d > 1.0e7) {
-    set_error("NUFFT (ragged): the grid is not f_k = (k0 + k) df with integer k0");
-    return LKB_E_UNSUPPORTED;
-  }
-  const int64_t k0 = (int64_t)k0d;
+  int64_t k0 = 0;
+  LKB_TRY(ragged_grid_check(B, h_span, f0, df, &k0));
   const int p = fine_log2(k0 + F), p2 = fine_log2(2 * (k0 + F));
   if (p2 > 24) { set_error("NUFFT (ragged): fine grid larger than 2^24 cells"); return LKB_E_UNSUPPORTED; }
-  for (int b = 0; b < B; ++b) {
-    if (!(h_span[b] > 0.0) || !(df * h_span[b] <= 1.0 + 1e-9)) {
-      set_error("NUFFT (ragged): a light curve has zero baseline or df * baseline > 1");
-      return LKB_E_UNSUPPORTED;
-    }
-  }
   const double sigma = fmin(2.0, nufft::grid_sigma(p, k0 + F));   // (the validated rule: beta = 2.30 w from sigma = 2 on)
   const int w = kernel_width(sigma);
   const float beta = (float)nufft::es_beta(w, sigma);
   const int64_t M = (int64_t)1 << p, M2 = (int64_t)1 << p2;
   const int npairs_all = (B + 1) / 2;
-  double cap_mb = 16384.0;
-  if (const char* e = getenv("LKB_NUFFT_RAGGED_MB")) { const double v = atof(e); if (v > 0.0) cap_mb = v; }
+  const double cap_mb = ragged_cap_mb();
   const double per_pair_mb = (2.0 * (double)M + 2.0 * (double)M2) * sizeof(float2) / 1048576.0;
   int group = (int)fmax(1.0, floor(cap_mb / per_pair_mb));
   if (group > npairs_all) group = npairs_all;
@@ -1350,7 +1476,7 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
   // v2 (one real transform per light curve, nufft_v2.cuh) when both fine grids are in range
   if (fft_mode(p) == 3 && fft_mode(p2) == 3)
     return ls_nufft_ragged_v2(d_t, d_y, d_off, d_po, B, ptotal, nmax, d_span, h_span, d_ysum, F, f0, df, k0, p, p2, w, beta,
-                              cap_mb, normalization, d_ns, d_pow, st);
+                              cap_mb, normalization, d_ns, d_pow, st, 0);
 
   Cad *cad = nullptr, *cad2 = nullptr;
   float2 *dec = nullptr, *dec2 = nullptr, *Za = nullptr, *Zb = nullptr, *Zw = nullptr;
@@ -1433,6 +1559,33 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
   }
   prof_end(st);
   return LKB_OK;
+}
+
+// Multi-term ("chi2", nterms in [1, 4]) periodogram of a ragged batch on one shared grid f_k = (k0 + k) df through the
+// v2 transforms: same inputs as ls_nufft_ragged_launch.  Harmonic j of every row is a mode of the same two transforms,
+// so the flux grid is sized for modes up to nterms (k0 + F) and the unit-strength grid for modes up to
+// 2 nterms (k0 + F); each row then solves its (2 nterms + 1)^2 normal equations in fp64.  Returns LKB_E_UNSUPPORTED
+// (the caller runs the direct kernel) when a light curve is not eligible (unsorted times, df * baseline > 1) or either
+// fine grid is outside the v2 range [2^14, 2^23].
+int ls_nufft_chi2_ragged_launch(const double* d_t, const float* d_y, const int64_t* d_off, const int64_t* d_po,
+                                const int64_t* h_off, int B, int64_t ptotal, int64_t nmax, const double* d_span,
+                                const double* h_span, const double* d_ysum, int64_t F, double f0, double df,
+                                int normalization, const double* d_ns, float* d_pow, cudaStream_t st, int nterms) {
+  (void)h_off;
+  if (nterms < 1 || nterms > 4) { set_error("NUFFT (ragged chi2): nterms must be in [1, 4]"); return LKB_E_ARG; }
+  int64_t k0 = 0;
+  LKB_TRY(ragged_grid_check(B, h_span, f0, df, &k0));
+  const int64_t kmax = (int64_t)nterms * (k0 + F);
+  const int p = fine_log2(kmax), p2 = fine_log2(2 * kmax);
+  if (p2 > V2R_P_MAX || fft_mode(p) != 3 || fft_mode(p2) != 3) {
+    set_error("NUFFT (ragged chi2): fine grids of 2^%d / 2^%d cells are outside the v2 transform's range", p, p2);
+    return LKB_E_UNSUPPORTED;
+  }
+  const double sigma = fmin(2.0, nufft::grid_sigma(p, kmax));
+  const int w = kernel_width(sigma);
+  const float beta = (float)nufft::es_beta(w, sigma);
+  return ls_nufft_ragged_v2(d_t, d_y, d_off, d_po, B, ptotal, nmax, d_span, h_span, d_ysum, F, f0, df, k0, p, p2, w, beta,
+                            ragged_cap_mb(), normalization, d_ns, d_pow, st, nterms);
 }
 
 }  // namespace lkb

@@ -184,14 +184,19 @@ def ls_power_ragged_device(t_cat, y_cat, offsets, frequency, normalization="ampl
 
 
 def ls_power_chi2(times, fluxes, frequency, nterms=1, normalization="amplitude", norm_scale=None,
-                  return_theta=False):
+                  return_theta=False, algo="auto"):
     """K1n.  Multi-term periodogram (astropy method="chi2"/"fastchi2", nterms in [1, 4]); same
     arguments as ls_power_ragged.  With return_theta also returns the 2*nterms+1 fitted parameters
-    per (light curve, frequency): [offset, sin 1, cos 1, sin 2, cos 2, ...]."""
+    per (light curve, frequency): [offset, sin 1, cos 1, sin 2, cos 2, ...].
+    `algo`: "auto" (the NUFFT kernels for a large job on one shared regular grid with sorted times and no theta, to
+    the parity tolerance of DESIGN.md section 2; else the direct sums), "direct" (always the exact fp64 direct sums)
+    or "nufft" (raises with status -5 when the grid, the times or return_theta do not qualify)."""
     lib = L.load()
     B = len(times)
     if B == 0:
         return []
+    if algo not in _RAGGED_ALGOS:
+        raise ValueError("algo must be one of %s" % sorted(_RAGGED_ALGOS))
     t, offsets = _csr(times)
     ydt = np.float32 if all(np.asarray(f).dtype == np.float32 for f in fluxes) else np.float64
     y, yoff = _csr(fluxes, ydt)
@@ -211,9 +216,9 @@ def ls_power_chi2(times, fluxes, frequency, nterms=1, normalization="amplitude",
         out = np.empty((B, F), dtype=np.float32)
         theta = np.empty((B, F, M), dtype=np.float64) if return_theta else None
     ns = None if norm_scale is None else np.ascontiguousarray(np.broadcast_to(norm_scale, (B,)), dtype=np.float64)
-    L.check(lib.lkb_ls_power_chi2(L.ptr(t), L.ptr(y), _y_dtype_code(ydt), L.ptr(offsets), B, L.ptr(freq), L.ptr(foff),
-                                  F, int(nterms), _NORMS[normalization], L.ptr(ns), L.ptr(out), L.ptr(theta),
-                                  L.MEM_HOST, None))
+    L.check(lib.lkb_ls_power_chi2_ex(L.ptr(t), L.ptr(y), _y_dtype_code(ydt), L.ptr(offsets), B, L.ptr(freq),
+                                     L.ptr(foff), F, int(nterms), _NORMS[normalization], L.ptr(ns), L.ptr(out),
+                                     L.ptr(theta), L.MEM_HOST, None, _RAGGED_ALGOS[algo]))
     if per_lc:
         out = [out[foff[b]:foff[b + 1]] for b in range(B)]
         if return_theta:

@@ -396,6 +396,10 @@ class LombScarglePeriodogram(Periodogram):
         direct sums or through a non-uniform FFT accurate to the parity tolerance (see ``_engine_algo``);
         the reference's default ``ls_method="fast"`` is astropy's coarser extirpolation + FFT approximation
         of the same quantity.  ``pg.ls_method`` records the requested/auto-switched name as in the reference.
+        The multi-term methods ``"chi2"``, ``"fastchi2"`` and ``"fastnifty_chi2"`` likewise let the library choose: a
+        large batch on a regular grid gets its harmonic sums from the non-uniform FFT, anything else exact direct sums,
+        both to the parity tolerance; ``engine.ls_power_chi2(..., algo="direct")`` forces the fp64
+        direct sums.
         """
         from . import engine
         prep = LombScarglePeriodogram._prepare(lc, **kwargs)
