@@ -222,6 +222,26 @@ int lkb_nanmedian_std(const double* x, const int64_t* offsets, int B,
 int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_lo, const int32_t* win_hi, int W,
                      double corr_factor, double* background, int mem, void* stream);
 
+/* ---- periodogram autocorrelation (seismology ACF2D) ------------------------------ */
+/* K7: the autocorrelations behind the numax and deltanu estimators, for many windows of many series in one call.
+ * Replaces seismology/utils.py:137-160 (autocorrelate), the per-numax loop of numax_estimators.py:170-182 and the
+ * autocorrelate call of deltanu_estimators.py.  For window k of series b (n = win_len[b] bins from win_start[k]):
+ *   y = x[start:start+n] - nanmean(x[start:start+n]),   acf_L = sum_{i < n-L} y_i y_{i+L}  (L = 0 .. n-1),
+ * i.e. np.correlate(y, y, "full")[n-1:], as exact fp64 direct sums (a NaN poisons exactly numpy's lags), and
+ *   metric[k] = (sum_L |acf_L| - 1) / n.
+ *   x           B ragged fp64 series back to back (x_offsets [B+1], HOST), e.g. the SNR power arrays
+ *   win_offsets [B+1] HOST CSR: the windows of series b are win_offsets[b] .. win_offsets[b+1]-1
+ *   win_start   [win_offsets[B]] HOST: first bin of each window inside its series
+ *   win_len     [B] HOST: window length (= lag count) of series b, >= 1
+ *   metric      [win_offsets[B]] fp64 out
+ *   acf         nullable fp64 out: per window win_len[b] lags, windows in order
+ * x, metric and acf follow `mem` (host mode is synchronous; device mode is asynchronous on `stream`).  A window's
+ * results are bitwise independent of the other windows of the batch and of the run.  LKB_E_ARG when a window leaves
+ * its series, a length is < 1, or a size is negative. */
+int lkb_acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets,
+                    const int64_t* win_start, const int64_t* win_len, double* metric, double* acf,
+                    int mem, void* stream);
+
 /* ---- multi-GPU: the one exchange step of the path (SURVEY.md 8e) ------------------ */
 /* A LightCurveCollection is sharded BY TARGET over one process per GPU; the only data exchange is the
  * reassembly of the fp32 power array [B, F] from the per-rank blocks (the reference has no counterpart: it

@@ -56,6 +56,7 @@ SIGNATURES = {
     "lkb_savgol_tables": (c_int, [c_int, c_int, c_vp, c_vp]),
     "lkb_nanmedian_std": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp]),
     "lkb_pg_logmedian": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_dbl, c_vp, c_int, c_vp]),
+    "lkb_acf_windows": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_nccl_version": (c_int, []),
     "lkb_nccl_unique_id": (c_int, [c_vp]),
     "lkb_nccl_init": (c_int, [c_int, c_int, c_vp]),

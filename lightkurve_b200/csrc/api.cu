@@ -222,6 +222,8 @@ int regress(const double*, int, const double*, const double*, const uint8_t*, co
             int64_t, int, double, int, double*, double*, uint8_t*, int32_t*, double*, int, cudaStream_t);
 int nanmedian_std(const double*, const int64_t*, int, double*, double*, int, cudaStream_t);
 int pg_logmedian(const double*, int, int64_t, const int32_t*, const int32_t*, int, double, double*, int, cudaStream_t);
+int acf_windows(const double*, const int64_t*, int, const int64_t*, const int64_t*, const int64_t*, double*, double*,
+                int, cudaStream_t);
 int savgol_tables_host(int, int, double*, double*);
 
 }  // namespace lkb
@@ -398,6 +400,13 @@ int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_l
                      double corr_factor, double* background, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return pg_logmedian(power, B, F, win_lo, win_hi, W, corr_factor, background, mem, (cudaStream_t)stream);
+}
+
+int lkb_acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets,
+                    const int64_t* win_start, const int64_t* win_len, double* metric, double* acf, int mem,
+                    void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return acf_windows(x, x_offsets, B, win_offsets, win_start, win_len, metric, acf, mem, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -9,8 +9,12 @@
 // reference's own expression (the x0 += 0.5 w accumulation must be reproduced in fp64); the GPU does the
 // B x W exact medians (K6 radix select, one CTA per (window, periodogram)) and the per-bin combination
 // in the reference's summation order (ascending window index).
+//
+// The seismology estimators that read the flattened periodogram (numax / deltanu ACF2D) run on the K7 windowed
+// autocorrelation kernels of acf.cuh; lkb_acf_windows enters through acf_windows below.
 #include "common.cuh"
 #include "select.cuh"
+#include "acf.cuh"
 
 namespace lkb {
 
@@ -110,6 +114,11 @@ int pg_logmedian(const double* power, int B, int64_t F, const int32_t* h_win_lo,
   LKB_TRY(stage_out_copy<double>(mem, bkg, d_b, (size_t)B * F, st));
   if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
   return LKB_OK;
+}
+
+int acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets, const int64_t* win_start,
+                const int64_t* win_len, double* metric, double* acf, int mem, cudaStream_t st) {
+  return acf_windows_launch(x, x_offsets, B, win_offsets, win_start, win_len, metric, acf, mem, st);
 }
 
 }  // namespace lkb

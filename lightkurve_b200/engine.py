@@ -497,6 +497,52 @@ def pg_logmedian(frequency, power, filter_width):
     return out[0] if one else out
 
 
+# bytes of series + outputs staged on the device by one lkb_acf_windows call; larger batches are split by series
+ACF_STAGE_BYTES = 2 << 30
+
+
+def acf_windows(series, starts, lengths, return_acf=False):
+    """K7.  Windowed autocorrelation (the seismology ACF2D step) of B series: `series` a list of 1-D arrays,
+    `starts` a list of int arrays (first bin of each window of series b), `lengths` a list of ints (the window
+    length = lag count of series b).  Window k of series b gives, with y = window - nanmean(window),
+    acf = np.correlate(y, y, "full")[n-1:] and metric = (sum |acf| - 1) / n.
+    Returns the list of metric arrays [n_windows_b] and, with return_acf, the list of [n_windows_b, n_b] acf arrays.
+    The batch goes to the GPU in groups of series whose staged input and output stay under ACF_STAGE_BYTES."""
+    lib = L.load()
+    B = len(series)
+    if len(starts) != B or len(lengths) != B:
+        raise ValueError("series, starts and lengths must have one entry per series")
+    xs = [np.asarray(s, dtype=np.float64).ravel() for s in series]
+    st = [np.asarray(s, dtype=np.int64).ravel() for s in starts]
+    ln = [int(n) for n in lengths]
+    cost = [8 * (len(x) + len(s) + (len(s) * n if return_acf else 0)) for x, s, n in zip(xs, st, ln)]
+    metrics, acfs = [None] * B, [None] * B
+    b0 = 0
+    while b0 < B:
+        b1, used = b0 + 1, cost[b0]
+        while b1 < B and used + cost[b1] <= ACF_STAGE_BYTES:
+            used += cost[b1]
+            b1 += 1
+        x, xoff = _csr(xs[b0:b1])
+        ws, woff = _csr(st[b0:b1], np.int64)
+        wl = np.ascontiguousarray(ln[b0:b1], dtype=np.int64)
+        W = int(woff[-1])
+        metric = np.empty(W, dtype=np.float64)
+        nlag = sum(len(s) * n for s, n in zip(st[b0:b1], ln[b0:b1]))
+        acf = np.empty(nlag, dtype=np.float64) if return_acf else None
+        L.check(lib.lkb_acf_windows(L.ptr(x), L.ptr(xoff), b1 - b0, L.ptr(woff), L.ptr(ws), L.ptr(wl),
+                                    L.ptr(metric), L.ptr(acf), L.MEM_HOST, None))
+        a0 = 0
+        for j, b in enumerate(range(b0, b1)):
+            metrics[b] = metric[woff[j]:woff[j + 1]]
+            if return_acf:
+                k = len(st[b])
+                acfs[b] = acf[a0:a0 + k * ln[b]].reshape(k, ln[b])
+                a0 += k * ln[b]
+        b0 = b1
+    return (metrics, acfs) if return_acf else metrics
+
+
 # --------------------------------------------------------------------------------------
 # multi-GPU exchange step (SURVEY.md 8e): NCCL all-gather through the C ABI
 # --------------------------------------------------------------------------------------

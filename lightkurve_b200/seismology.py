@@ -7,6 +7,9 @@ background, K6); the estimators themselves work on the resulting signal-to-noise
 reference: numax by the 2-D autocorrelation ("ACF2D") collapsed metric, deltanu by the autocorrelation of the
 mode envelope, radius / mass / logg by the solar scaling relations with first-order error propagation (the
 reference uses the `uncertainties` package for that; the formulae below are its linear propagation written out).
+``estimate_numax_acf2d_batch`` / ``estimate_deltanu_acf2d_batch`` give the same results for many periodograms with
+every autocorrelation in one GPU pass (K7, ``engine.acf_windows``); validation, window placement and the final
+smoothing / peak search are the same functions as the per-periodogram estimators'.
 Plotting / echelle diagrams are out of scope.
 """
 import logging
@@ -22,7 +25,7 @@ from .utils import LightkurveWarning, validate_method
 log = logging.getLogger(__name__)
 
 __all__ = ["Seismology", "SeismologyQuantity", "estimate_numax_acf2d", "estimate_deltanu_acf2d",
-           "estimate_radius", "estimate_mass", "estimate_logg", "NUMAX_SOL", "DELTANU_SOL", "TEFF_SOL", "G_SOL"]
+           "estimate_numax_acf2d_batch", "estimate_deltanu_acf2d_batch", "estimate_radius", "estimate_mass", "estimate_logg", "NUMAX_SOL", "DELTANU_SOL", "TEFF_SOL", "G_SOL"]
 
 
 class _UFloat:
@@ -81,17 +84,36 @@ def get_fwhm(periodogram, numax):
     return 0.66 * numax ** 0.88
 
 
+def _window_slices(F, f0, numaxs, window_width, fs):
+    """(start, length) arrays of the reference's windows ``power[centre - spread : centre + spread]`` with
+    spread = int(window_width / 2 / fs) and centre = int(numax / fs) - int(f0 / fs) (the same fp64 expressions,
+    truncated toward zero like int()), under Python's slice rules: a negative end counts from the end of the
+    array, then both ends are clipped to [0, F]; the slice may come out truncated or empty."""
+    spread = int(window_width / 2 / fs)
+    centre = np.trunc(np.asarray(numaxs, dtype=float) / fs).astype(np.int64) - int(f0 / fs)
+
+    def resolve(e):
+        return np.where(e < 0, np.maximum(e + F, 0), np.minimum(e, F))
+
+    start, stop = resolve(centre - spread), resolve(centre + spread)
+    return start, np.maximum(stop - start, 0)
+
+
+def _correlate(sel):
+    """Non-negative lags of the autocorrelation of the mean-subtracted window (np.correlate "full")."""
+    sel = np.array(sel, dtype=float)
+    sel -= np.nanmean(sel)
+    return np.correlate(sel, sel, mode="full")[len(sel) - 1:]
+
+
 def autocorrelate(periodogram, numax, window_width=25.0, frequency_spacing=None):
     """Autocorrelation (non-negative lags) of the mean-subtracted power in a window of `window_width` around
     `numax` (both in the periodogram's frequency unit)."""
     freq = np.asarray(periodogram.frequency.value, dtype=float)
     if frequency_spacing is None:
         frequency_spacing = np.median(np.diff(freq))
-    spread = int(window_width / 2 / frequency_spacing)
-    centre = int(numax / frequency_spacing) - int(freq[0] / frequency_spacing)
-    sel = np.array(np.asarray(periodogram.power.value, dtype=float)[centre - spread: centre + spread])
-    sel -= np.nanmean(sel)
-    return np.correlate(sel, sel, mode="full")[len(sel) - 1:]
+    start, length = _window_slices(len(freq), freq[0], [numax], window_width, frequency_spacing)
+    return _correlate(np.asarray(periodogram.power.value, dtype=float)[start[0]:start[0] + length[0]])
 
 
 def _gaussian_smooth_extend(x, stddev):
@@ -107,12 +129,22 @@ def _gaussian_smooth_extend(x, stddev):
     return np.convolve(padded, kernel, mode="valid")
 
 
-# ---- numax (seismology/numax_estimators.py:15-215) ---------------------------------------------------
-def estimate_numax_acf2d(periodogram, numaxs=None, window_width=None, spacing=None):
-    """numax = centre of the window whose autocorrelation carries the most (smoothed) collapsed power."""
+def _check_evenly_spaced(periodogram):
     if not periodogram._is_evenly_spaced():
         raise ValueError("the ACF 2D method requires that the periodogram "
                          "has a grid of uniformly spaced frequencies.")
+
+
+def _which(index):
+    return "" if index is None else " (periodogram {})".format(index)
+
+
+# ---- numax (seismology/numax_estimators.py:15-215) ---------------------------------------------------
+def _numax_setup(periodogram, numaxs, window_width, spacing, index=None):
+    """Validation and window placement of the ACF2D numax estimator: the trial numaxs, the window width, the
+    lag count and the first bin of every window.  A window the reference's slice would truncate (or leave empty)
+    makes its loop fail; it raises ValueError here, before any autocorrelation."""
+    _check_evenly_spaced(periodogram)
     funit = periodogram.frequency.unit
     freq = np.asarray(periodogram.frequency.value, dtype=float)
     main_sequence = _in_microhertz(periodogram.frequency[-1]) > 500.0
@@ -139,29 +171,66 @@ def estimate_numax_acf2d(periodogram, numaxs=None, window_width=None, spacing=No
     if np.any(numaxs > np.nanmax(freq)):
         raise ValueError("A custom range of numaxs can not extend above "
                          "the highest frequency value in the periodogram.")
+    if len(numaxs) == 0:
+        raise ValueError("No trial numax fits in the periodogram{}.".format(_which(index)))
     nlags = int(window_width / 2 / fs) * 2
-    acf2d = np.zeros([nlags, len(numaxs)])
-    metric = np.zeros(len(numaxs))
-    for idx, numax in enumerate(numaxs):
-        acf = autocorrelate(periodogram, numax, window_width=window_width, frequency_spacing=fs)
-        acf2d[:, idx] = acf
-        metric[idx] = (np.sum(np.abs(acf)) - 1) / len(acf)
+    starts, lengths = _window_slices(len(freq), freq[0], numaxs, window_width, fs)
+    bad = np.flatnonzero(lengths != nlags) if nlags >= 1 else [0]
+    if len(bad):
+        raise ValueError("The {}-bin window around numax = {} {} does not fit in the periodogram{}.".format(
+            nlags, numaxs[bad[0]], funit.to_string(), _which(index)))
+    return dict(funit=funit, power=np.asarray(periodogram.power.value, dtype=float), numaxs=numaxs,
+                window_width=window_width, nlags=nlags, starts=starts)
+
+
+def _numax_finish(setup, metric, acf2d):
+    """numax = the trial numax of the largest smoothed metric; the diagnostics of the reference."""
+    numaxs = setup["numaxs"]
     if len(numaxs) > 10:
         metric_smooth = _gaussian_smooth_extend(metric, np.sqrt(len(numaxs)))
     else:
         metric_smooth = metric
-    best = Quantity(numaxs[np.argmax(metric_smooth)], funit)
-    diagnostics = {"numaxs": numaxs, "acf2d": acf2d, "window_width": window_width, "metric": metric,
+    best = Quantity(numaxs[np.argmax(metric_smooth)], setup["funit"])
+    diagnostics = {"numaxs": numaxs, "acf2d": acf2d, "window_width": setup["window_width"], "metric": metric,
                    "metric_smooth": metric_smooth}
     return SeismologyQuantity(best, name="numax", method="ACF2D", diagnostics=diagnostics)
 
 
+def estimate_numax_acf2d(periodogram, numaxs=None, window_width=None, spacing=None):
+    """numax = centre of the window whose autocorrelation carries the most (smoothed) collapsed power."""
+    setup = _numax_setup(periodogram, numaxs, window_width, spacing)
+    nlags, power = setup["nlags"], setup["power"]
+    acf2d = np.zeros([nlags, len(setup["numaxs"])])
+    metric = np.zeros(len(setup["numaxs"]))
+    for idx, start in enumerate(setup["starts"]):
+        acf = _correlate(power[start:start + nlags])
+        acf2d[:, idx] = acf
+        metric[idx] = (np.sum(np.abs(acf)) - 1) / len(acf)
+    return _numax_finish(setup, metric, acf2d)
+
+
+def estimate_numax_acf2d_batch(periodograms, numaxs=None, window_width=None, spacing=None, return_acf2d=False):
+    """`estimate_numax_acf2d` of many periodograms with every autocorrelation in one GPU pass (K7,
+    ``engine.acf_windows``).  Element b equals ``estimate_numax_acf2d(periodograms[b], numaxs, window_width,
+    spacing)``: value, unit and diagnostics.  The diagnostic "acf2d" ([nlags, len(numaxs)]) is only filled with
+    `return_acf2d` (a catalog of red giants at oversample 5 holds tens of GB of it); otherwise it is None.
+    Every periodogram is validated before the GPU runs; a failure raises the loop's ValueError."""
+    from . import engine
+    setups = [_numax_setup(pg, numaxs, window_width, spacing, index=b) for b, pg in enumerate(periodograms)]
+    if not setups:
+        return []
+    res = engine.acf_windows([s["power"] for s in setups], [s["starts"] for s in setups],
+                             [s["nlags"] for s in setups], return_acf=return_acf2d)
+    metrics, acfs = res if return_acf2d else (res, [None] * len(setups))
+    return [_numax_finish(s, np.asarray(m), None if a is None else np.asarray(a).T)
+            for s, m, a in zip(setups, metrics, acfs)]
+
+
 # ---- deltanu (seismology/deltanu_estimators.py:15-129) -------------------------------------------------
-def estimate_deltanu_acf2d(periodogram, numax):
-    """deltanu = the autocorrelation peak of the mode envelope closest to 0.294 numax^0.772 (Stello et al. 2009)."""
-    if not periodogram._is_evenly_spaced():
-        raise ValueError("the ACF 2D method requires that the periodogram "
-                         "has a grid of uniformly spaced frequencies.")
+def _deltanu_setup(periodogram, numax, index=None):
+    """Validation and window placement of the ACF2D deltanu estimator.  The reference's slice may be truncated
+    by the end of the spectrum (a shorter autocorrelation); an empty one makes it fail and raises ValueError."""
+    _check_evenly_spaced(periodogram)
     funit = periodogram.frequency.unit
     freq = np.asarray(periodogram.frequency.value, dtype=float)
     numax = Quantity(numax, funit)
@@ -174,15 +243,49 @@ def estimate_deltanu_acf2d(periodogram, numax):
                          "the highest frequency value in the periodogram.")
     deltanu_emp = float(np.asarray(Quantity(0.294 * _in_microhertz(numax) ** 0.772, u.microhertz).to(funit).value))
     window_width = 2 * int(np.floor(get_fwhm(periodogram, numax_value)))
-    aacf = autocorrelate(periodogram, numax=numax_value, window_width=window_width)
+    start, length = (int(v[0]) for v in _window_slices(len(freq), freq[0], [numax_value], window_width, fs))
+    if length < 1:
+        raise ValueError("The window around numax = {} {} is empty{}.".format(numax_value, funit.to_string(),
+                                                                               _which(index)))
+    return dict(funit=funit, power=np.asarray(periodogram.power.value, dtype=float), numax=numax, fs=fs,
+                deltanu_emp=deltanu_emp, start=start, length=length)
+
+
+def _deltanu_finish(setup, aacf):
+    """deltanu = the autocorrelation peak closest to the empirical deltanu; the diagnostics of the reference."""
+    fs, deltanu_emp = setup["fs"], setup["deltanu_emp"]
     acf = (np.abs(aacf ** 2) / np.abs(aacf[0] ** 2)) / (3 / (2 * len(aacf)))
     lags = np.linspace(0.0, len(acf) * fs, len(acf))
     sel = (lags > 0.75 * deltanu_emp) & (lags < 1.25 * deltanu_emp)
     peaks, _ = find_peaks(acf[sel], distance=np.floor(deltanu_emp / 2.0 / fs))
     candidates = lags[sel][peaks]
-    best = Quantity(candidates[np.argmin(np.abs(candidates - deltanu_emp))], funit)
-    diagnostics = {"lags": lags, "acf": acf, "peaks": peaks, "sel": sel, "numax": numax, "deltanu_emp": deltanu_emp}
+    best = Quantity(candidates[np.argmin(np.abs(candidates - deltanu_emp))], setup["funit"])
+    diagnostics = {"lags": lags, "acf": acf, "peaks": peaks, "sel": sel, "numax": setup["numax"],
+                   "deltanu_emp": deltanu_emp}
     return SeismologyQuantity(best, name="deltanu", method="ACF2D", diagnostics=diagnostics)
+
+
+def estimate_deltanu_acf2d(periodogram, numax):
+    """deltanu = the autocorrelation peak of the mode envelope closest to 0.294 numax^0.772 (Stello et al. 2009)."""
+    setup = _deltanu_setup(periodogram, numax)
+    start, length = setup["start"], setup["length"]
+    return _deltanu_finish(setup, _correlate(setup["power"][start:start + length]))
+
+
+def estimate_deltanu_acf2d_batch(periodograms, numaxs):
+    """`estimate_deltanu_acf2d` of many (periodogram, numax) pairs with the autocorrelations in one GPU pass (K7,
+    ``engine.acf_windows``); the peak search stays on the host.  Element b equals
+    ``estimate_deltanu_acf2d(periodograms[b], numaxs[b])``."""
+    from . import engine
+    if len(numaxs) != len(periodograms):
+        raise ValueError("Pass one numax per periodogram ({} periodograms, {} numaxs).".format(
+            len(periodograms), len(numaxs)))
+    setups = [_deltanu_setup(pg, nm, index=b) for b, (pg, nm) in enumerate(zip(periodograms, numaxs))]
+    if not setups:
+        return []
+    _, acfs = engine.acf_windows([s["power"] for s in setups], [[s["start"]] for s in setups],
+                                 [s["length"] for s in setups], return_acf=True)
+    return [_deltanu_finish(s, np.asarray(a)[0]) for s, a in zip(setups, acfs)]
 
 
 # ---- scaling relations (seismology/stellar_estimators.py) ----------------------------------------------
