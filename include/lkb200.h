@@ -238,6 +238,21 @@ int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_l
  * x, metric and acf follow `mem` (host mode is synchronous; device mode is asynchronous on `stream`).  A window's
  * results are bitwise independent of the other windows of the batch and of the run.  LKB_E_ARG when a window leaves
  * its series, a length is < 1, or a size is negative. */
+/* ---- CBVCorrector.correct_elasticnet --------------------------------------- */
+/* K8: sklearn.linear_model.ElasticNet(alpha, l1_ratio, fit_intercept=False).fit(X[mask], y[mask]) and the model of
+ * correctors/cbvcorrector.py:358-379, for B light curves in one call.  The coordinate descent reproduces
+ * scikit-learn's iteration (cyclic order, stopping rule, gap-safe screening), not just its minimiser.
+ *   X            [N,K] row-major fp64, shared by the batch (x_batched=0) or [B,N,K] (x_batched=1)
+ *   y            [B,N] fp64;  cadence_mask uint8 [B,N] or NULL (1 = use; NULL = all)
+ *   alpha >= 0, 0 <= l1_ratio <= 1, max_iter >= 1, tol >= 0, positive 0/1: ElasticNet's parameters
+ *   outputs: coeff [B,K] (coef_), model [B,N] = X[:, :-1] coef[:-1] minus its median over all N cadences,
+ *            n_iter int32 [B] (n_iter_), dual_gap [B] (dual_gap_), converged uint8 [B] (0: scikit-learn would
+ *            raise its ConvergenceWarning)
+ * LKB_E_ARG for a parameter out of range or a light curve without a used cadence, LKB_E_UNSUPPORTED for K > 165. */
+int lkb_elasticnet(const double* X, int x_batched, const double* y, const uint8_t* cadence_mask, int B, int64_t N,
+                   int K, double alpha, double l1_ratio, int max_iter, double tol, int positive, double* coeff,
+                   double* model, int32_t* n_iter, double* dual_gap, uint8_t* converged, int mem, void* stream);
+
 int lkb_acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets,
                     const int64_t* win_start, const int64_t* win_len, double* metric, double* acf,
                     int mem, void* stream);

@@ -4,14 +4,16 @@ Lomb-Scargle over-fitting metric (K1) inside a bounded scalar optimiser (SURVEY.
 
 Scope: everything that runs from arrays - the basis-vector container (`to_designmatrix`, `align`, `interpolate`),
 `correct_gaussian_prior`, the `correct` optimiser over the regularisation `alpha`, `over_fitting_metric`,
-`correct_regressioncorrector`.  Out of scope here: reading CBV FITS files / downloading them from MAST
-(`load_kepler_cbvs`, `load_tess_cbvs`), the under-fitting metric (it needs a MAST search of neighbouring targets),
-`correct_elasticnet` (scikit-learn's coordinate descent, not on the hot path) and the plots.  Basis vectors are
+`correct_regressioncorrector`, and `correct_elasticnet` (scikit-learn's elastic-net coordinate descent, K8; with
+`correct_elasticnet_batch` for many correctors in one call).  Out of scope here: reading CBV FITS files / downloading
+them from MAST (`load_kepler_cbvs`, `load_tess_cbvs`), the under-fitting metric (it needs a MAST search of
+neighbouring targets) and the plots.  Basis vectors are
 therefore handed over explicitly (``CBVCorrector(lc, cbvs=[...])``, an extension of the reference signature) or
 left out (``do_not_load_cbvs=True`` with an external design matrix, as in the reference's own non-remote test).
 """
 import copy
 import logging
+import warnings
 
 import numpy as np
 from scipy.interpolate import PchipInterpolator
@@ -26,7 +28,50 @@ from .regressioncorrector import RegressionCorrector
 
 log = logging.getLogger(__name__)
 
-__all__ = ["CBVCorrector", "CotrendingBasisVectors"]
+__all__ = ["CBVCorrector", "CotrendingBasisVectors", "ConvergenceWarning"]
+
+
+class ConvergenceWarning(UserWarning):
+    """The elastic-net coordinate descent stopped on `max_iter` before its duality gap reached the tolerance
+    (scikit-learn's `sklearn.exceptions.ConvergenceWarning`, with the same text)."""
+
+
+MESSAGE_ALPHA0 = ("With alpha=0, this algorithm does not converge well. You are advised to use the LinearRegression "
+                  "estimator")
+_ENET_FORWARDED = {"max_iter": 1000, "tol": 1e-4, "positive": False}
+_ENET_NO_EFFECT = ("precompute", "copy_X", "warm_start", "random_state")
+
+
+def _convergence_message(gap, tol, l1):
+    msg = ("Objective did not converge. You might want to increase the number of iterations, check the scale of the "
+           "features or consider increasing regularisation. Duality gap: {:.6e}, tolerance: {:.3e}".format(gap, tol))
+    if l1 < np.finfo(np.float64).eps:
+        msg += ("\nLinear regression models with a zero l1 penalization strength are more efficiently fitted using "
+                "one of the solvers implemented in sklearn.linear_model.Ridge/RidgeCV instead.")
+    return msg
+
+
+def _elasticnet_options(kwargs):
+    """ElasticNet keyword arguments -> the kernel's max_iter / tol / positive."""
+    opts = dict(_ENET_FORWARDED)
+    for key, value in kwargs.items():
+        if key in _ENET_FORWARDED:
+            opts[key] = value
+        elif key == "selection":
+            if value == "random":
+                raise NotImplementedError("selection='random' is not available: the GPU fit is cyclic")
+            if value != "cyclic":
+                raise ValueError("selection must be 'cyclic' or 'random', got {!r}".format(value))
+        elif key not in _ENET_NO_EFFECT:
+            raise TypeError("correct_elasticnet() got an unexpected keyword argument {!r}".format(key))
+    opts["positive"] = bool(opts["positive"])
+    return opts
+
+
+def _per_item(value, n):
+    """True when `value` is a list/tuple with one design matrix / mask (or None) per corrector."""
+    return (isinstance(value, (list, tuple)) and len(value) == n and
+            all(v is None or isinstance(v, DesignMatrix) or np.ndim(v) == 1 for v in value))
 
 
 class CotrendingBasisVectors:
@@ -230,6 +275,79 @@ class CBVCorrector(RegressionCorrector):
         self.correct_regressioncorrector(self.design_matrix_collection, cadence_mask=cadence_mask, **kwargs)
         self.alpha = alpha
         return self.corrected_lc
+
+    # ---- elastic net (cbvcorrector.py:294-395): scikit-learn's coordinate descent, one lkb_elasticnet call ----
+    def correct_elasticnet(self, cbv_type='SingleScale', cbv_indices=np.arange(1, 9), alpha=1e-20, l1_ratio=0.01,
+                           ext_dm=None, cadence_mask=None, **kwargs):
+        """Fit with combined L1 and L2 penalties: the coefficients of
+        ``sklearn.linear_model.ElasticNet(alpha, l1_ratio, fit_intercept=False, **kwargs).fit(X[mask], y[mask])``,
+        reproduced iteration for iteration on the GPU (K8).  The model leaves out the constant column and is
+        median-subtracted, so the corrected light curve keeps the flux's median.  `alpha` does not scale like the
+        `alpha` of `correct_gaussian_prior`.
+
+        Keyword arguments of ElasticNet: `max_iter`, `tol` and `positive` are honoured; `precompute`, `copy_X`,
+        `warm_start` and `random_state` do not change a fresh cyclic fit and are accepted; `selection="random"` is not
+        available.  A fit that stops on `max_iter` warns with ElasticNet's `ConvergenceWarning` text."""
+        self._correct_initialization(cbv_type=cbv_type, cbv_indices=cbv_indices, ext_dm=ext_dm)
+        CBVCorrector._run_elasticnet([self], [cadence_mask], alpha, l1_ratio, _elasticnet_options(kwargs))
+        return self.corrected_lc
+
+    @staticmethod
+    def correct_elasticnet_batch(correctors, cbv_type='SingleScale', cbv_indices=np.arange(1, 9), alpha=1e-20,
+                                 l1_ratio=0.01, ext_dm=None, cadence_mask=None, **kwargs):
+        """`correct_elasticnet` for many correctors in as few GPU calls as possible: one call with a shared design
+        matrix when every corrector's matrix is the same, one call per group of equal-shaped matrices otherwise.
+        `ext_dm` and `cadence_mask` are either shared or lists with one entry per corrector.  Every corrector ends in
+        the state its own `correct_elasticnet` call would leave; returns the list of corrected light curves."""
+        correctors = list(correctors)
+        B = len(correctors)
+        ext = ext_dm if _per_item(ext_dm, B) else [ext_dm] * B
+        masks = cadence_mask if _per_item(cadence_mask, B) else [cadence_mask] * B
+        opts = _elasticnet_options(kwargs)
+        for c, e in zip(correctors, ext):
+            c._correct_initialization(cbv_type=cbv_type, cbv_indices=cbv_indices, ext_dm=e)
+        CBVCorrector._run_elasticnet(correctors, masks, alpha, l1_ratio, opts)
+        return [c.corrected_lc for c in correctors]
+
+    @staticmethod
+    def _run_elasticnet(correctors, masks, alpha, l1_ratio, opts):
+        from .. import engine
+        Xs, ys, ms = [], [], []
+        for c, m in zip(correctors, masks):
+            X = np.ascontiguousarray(c.design_matrix_collection.values, dtype=np.float64)
+            if not np.all(np.isfinite(X)):
+                raise ValueError("Input X contains NaN or infinity.")
+            n = len(c.lc.flux)
+            m = np.ones(n, bool) if m is None else np.asarray(m, dtype=bool)
+            if m.shape != (n,):
+                raise ValueError("cadence_mask must have one entry per cadence")
+            Xs.append(X)
+            ys.append(np.asarray(c.lc.flux.value, dtype=np.float64))
+            ms.append(m)
+        if alpha == 0:
+            warnings.warn(MESSAGE_ALPHA0, UserWarning, stacklevel=3)
+        groups = {}
+        for b, X in enumerate(Xs):
+            groups.setdefault(X.shape, []).append(b)
+        for idx in groups.values():
+            shared = all(Xs[b] is Xs[idx[0]] or np.array_equal(Xs[b], Xs[idx[0]]) for b in idx)
+            X = Xs[idx[0]] if shared else np.stack([Xs[b] for b in idx])
+            res = engine.elasticnet(X, np.stack([ys[b] for b in idx]), np.stack([ms[b] for b in idx]), alpha=alpha,
+                                    l1_ratio=l1_ratio, **opts)
+            for j, b in enumerate(idx):
+                c, m = correctors[b], ms[b]
+                if not res["converged"][j]:
+                    n = int(np.count_nonzero(m))
+                    ym = ys[b][m]
+                    warnings.warn(_convergence_message(res["dual_gap"][j] * n, opts["tol"] * float(ym @ ym),
+                                                       alpha * l1_ratio * n), ConvergenceWarning, stacklevel=3)
+                c.coefficients = res["coefficients"][j]
+                c.coefficients_err = None
+                c.elasticnet_n_iter = int(res["n_iter"][j])
+                c.elasticnet_dual_gap = float(res["dual_gap"][j])
+                c._finish(res["model"][j])
+                c.cadence_mask = m
+                c.alpha = alpha
 
     def correct(self, cbv_type=["SingleScale"], cbv_indices=[np.arange(1, 9)], ext_dm=None, cadence_mask=None,
                 alpha_bounds=[1e-4, 1e4], target_over_score=0.5, target_under_score=0.5, max_iter=100):

@@ -220,6 +220,8 @@ int flatten(const double*, const double*, const double*, const uint8_t*, const i
             double, double*, double*, double*, int, cudaStream_t);
 int regress(const double*, int, const double*, const double*, const uint8_t*, const double*, const double*, int,
             int64_t, int, double, int, double*, double*, uint8_t*, int32_t*, double*, int, cudaStream_t);
+int elasticnet(const double*, int, const double*, const uint8_t*, int, int64_t, int, double, double, int, double, int,
+               double*, double*, int32_t*, double*, uint8_t*, int, cudaStream_t);
 int nanmedian_std(const double*, const int64_t*, int, double*, double*, int, cudaStream_t);
 int pg_logmedian(const double*, int, int64_t, const int32_t*, const int32_t*, int, double, double*, int, cudaStream_t);
 int acf_windows(const double*, const int64_t*, int, const int64_t*, const int64_t*, const int64_t*, double*, double*,
@@ -384,6 +386,14 @@ int lkb_regress(const double* X, int x_batched, const double* y, const double* f
   std::lock_guard<std::mutex> lk(g_mu);
   return regress(X, x_batched, y, flux_err, cadence_mask, prior_mu, prior_sigma, B, N, K, clip_sigma, niters, coeff,
                  model, outlier_mask, status_out, coeff_cov, mem, (cudaStream_t)stream);
+}
+
+int lkb_elasticnet(const double* X, int x_batched, const double* y, const uint8_t* cadence_mask, int B, int64_t N,
+                   int K, double alpha, double l1_ratio, int max_iter, double tol, int positive, double* coeff,
+                   double* model, int32_t* n_iter, double* dual_gap, uint8_t* converged, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return elasticnet(X, x_batched, y, cadence_mask, B, N, K, alpha, l1_ratio, max_iter, tol, positive, coeff, model,
+                    n_iter, dual_gap, converged, mem, (cudaStream_t)stream);
 }
 
 int lkb_savgol_tables(int window_length, int polyorder, double* coeffs, double* edge) {

@@ -14,7 +14,10 @@
 //           rg_solve    add the Gaussian priors, LU with partial pivoting in shared memory (gesv-like)
 //           rg_clip     model = X w, residuals, astropy sigma_clip (median / std, <= 5 rounds)
 //           rg_final    model - median(model)
+//
+// K8 (lkb_elasticnet, enet.cuh) reuses rg_rows + the fp64 Gram pass and rg_final: see elasticnet() below.
 #include "common.cuh"
+#include "enet.cuh"
 #include "select.cuh"
 
 namespace lkb {
@@ -729,6 +732,53 @@ __global__ void rg_zero_kernel(double* p, int64_t n, uint8_t* q, int64_t nq) {
   if (q && i < nq) q[i] = 0;
 }
 
+// The exact fp64 Gram pass over the listed rows: the FP64 tensor-core kernel when its tiling covers K + 1 columns,
+// else the SIMT kernel (LKB_REGRESS_SIMT=1 forces the SIMT kernel, kept for A/B measurements).  `sign` +1 adds the
+// rows, -1 removes them; `first` marks the first pass of a call (it may split a light curve over two CTAs).
+// Shared by lkb_regress and lkb_elasticnet.
+static int rg_gram_pass(const double* d_X, int x_batched, const double* d_y, const double* d_fe, int B, int64_t N,
+                        int K, double sign, bool first, RgWs ws, cudaStream_t st) {
+  const int Ka = K + 1;
+  const int ntile = (Ka + 7) / 8;
+  const int tb = ntile <= 20 ? 4 : 5;
+  const int nb5 = (ntile + tb - 1) / tb;
+  static const bool force_simt = getenv("LKB_REGRESS_SIMT") != nullptr;
+  const bool use_mma = !force_simt && Ka <= RGM_LD && nb5 <= 5;
+  static bool attr = false;
+  if (!attr) {
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_accum_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)(2 * sizeof(RgStage))));
+    const int sm2 = (int)(2 * sizeof(RgmStage));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<3, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<5, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<5, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
+    attr = true;
+  }
+  if (use_mma) {
+    const size_t sm2 = 2 * sizeof(RgmStage);
+    // first pass of a small batch: two CTAs per light curve to fill the SMs (wave quantisation)
+    const dim3 g((unsigned)B, (first && B < 4 * sm_count() && N >= 4096) ? 2u : 1u);
+    const unsigned nt = 32u * nb5 * (nb5 + 1) / 2;
+    if (tb == 5) rg_gram_mma_kernel<5, 5><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws);
+    else switch (nb5) {
+      case 1: rg_gram_mma_kernel<1, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws); break;
+      case 2: rg_gram_mma_kernel<2, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws); break;
+      case 3: rg_gram_mma_kernel<3, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws); break;
+      case 4: rg_gram_mma_kernel<4, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws); break;
+      default: rg_gram_mma_kernel<5, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws); break;
+    }
+  } else {
+    const int nblk = (Ka + RG_BLK - 1) / RG_BLK;
+    const int nupper = nblk * (nblk + 1) / 2;
+    rg_accum_kernel<<<dim3(nupper, B), 128, 2 * sizeof(RgStage), st>>>(d_X, x_batched, d_y, d_fe, N, K, nblk, sign,
+                                                                         ws);
+  }
+  return LKB_OK;
+}
+
 bool regress_tc_supported(int B, int64_t N, int K);                                              // regress_tc.cu
 int regress_tc_gram(const double* d_X, const double* d_y, const double* d_fe, const uint8_t* d_used, int B, int64_t N,
                     int K, double* d_gram, cudaStream_t st);
@@ -782,8 +832,6 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
     rg_zero_kernel<<<(unsigned)((nz + 255) / 256), 256, 0, st>>>(ws.gram, ng, o_om, (int64_t)BN);
     LKB_LAUNCH_CHECK();
   }
-  const int nblk = (Ka + RG_BLK - 1) / RG_BLK;
-  const int nupper = nblk * (nblk + 1) / 2;
   const size_t solve_smem = (size_t)K * Ka * sizeof(double);
   static size_t solve_attr = 0;
   if (solve_smem > solve_attr) {
@@ -791,30 +839,10 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
     LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem));
     solve_attr = solve_smem;
   }
-  static bool accum_attr = false;
-  if (!accum_attr) {
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_accum_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)(2 * sizeof(RgStage))));
-    accum_attr = true;
-  }
-  // FP64 tensor-core Gram kernel (default) / SIMT kernel (LKB_REGRESS_SIMT=1, kept for A/B measurements)
-  const int ntile = (Ka + 7) / 8;
-  const int tb = ntile <= 20 ? 4 : 5;
-  const int nb5 = (ntile + tb - 1) / tb;
+  // the first Gram pass of a large shared-design-matrix batch may take the tcgen05 GEMM; every other pass takes the
+  // exact fp64 kernels of rg_gram_pass (LKB_REGRESS_SIMT=1: SIMT kernels throughout, kept for A/B measurements)
   static const bool force_simt = getenv("LKB_REGRESS_SIMT") != nullptr;
-  const bool use_mma = !force_simt && Ka <= RGM_LD && nb5 <= 5;
   const bool use_tc = !force_simt && !x_batched && regress_tc_supported(B, N, K);
-  static bool mma_attr = false;
-  if (!mma_attr) {
-    const int sm2 = (int)(2 * sizeof(RgmStage));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<3, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<5, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    LKB_CUDA_CHECK(cudaFuncSetAttribute(rg_gram_mma_kernel<5, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm2));
-    mma_attr = true;
-  }
   // batched model X w as one FP64 tensor-core GEMM when the design matrix is shared by the batch
   const bool gemm_model = !force_simt && !x_batched && K <= RGM_LD - 1 && B >= 8;
   dim3 gemm_grid(1, (unsigned)((B + RGE_LC - 1) / RGE_LC));
@@ -843,23 +871,9 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
     if (it == 0 && use_tc) {
       // first fit of a large shared-design-matrix batch: the Gram matrices as one tcgen05 GEMM (regress_tc.cu)
       LKB_TRY(regress_tc_gram(d_X, d_y, d_fe, ws.used, B, N, K, ws.gram, st));
-    } else if (use_mma) {
-      const double sgn = it == 0 ? 1.0 : -1.0;
-      const size_t sm2 = 2 * sizeof(RgmStage);
-      // first pass of a small batch: two CTAs per light curve to fill the SMs (wave quantisation)
-      const dim3 g((unsigned)B, (it == 0 && B < 4 * sm_count() && N >= 4096) ? 2u : 1u);
-      const unsigned nt = 32u * nb5 * (nb5 + 1) / 2;
-      if (tb == 5) rg_gram_mma_kernel<5, 5><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws);
-      else switch (nb5) {
-        case 1: rg_gram_mma_kernel<1, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws); break;
-        case 2: rg_gram_mma_kernel<2, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws); break;
-        case 3: rg_gram_mma_kernel<3, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws); break;
-        case 4: rg_gram_mma_kernel<4, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws); break;
-        default: rg_gram_mma_kernel<5, 4><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sgn, ws); break;
-      }
-    } else
-      rg_accum_kernel<<<dim3(nupper, B), 128, 2 * sizeof(RgStage), st>>>(d_X, x_batched, d_y, d_fe, N, K, nblk,
-                                                                           it == 0 ? 1.0 : -1.0, ws);
+    } else {
+      LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, d_fe, B, N, K, it == 0 ? 1.0 : -1.0, it == 0, ws, st));
+    }
     if (it == 0) { prof_end(st); prof_begin(st); }     // second record: everything after the first Gram pass
     LKB_LAUNCH_CHECK();
     double* d_lu = nullptr;
@@ -914,6 +928,100 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
   LKB_TRY(stage_out_copy<uint8_t>(mem, outlier_mask, o_om, BN, st));
   LKB_TRY(stage_out_copy<int32_t>(mem, status_out, o_st, B, st));
   LKB_TRY(stage_out_copy<double>(mem, coeff_cov, o_cov, (size_t)B * K * K, st));
+  if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LKB_OK;
+}
+
+// K8: CBVCorrector.correct_elasticnet (cbvcorrector.py:358-379).  The unit-weight Gram matrix [X | y]^T M [X | y] of
+// the used cadences (K5's first pass, always the exact fp64 kernels: the ~1e-6 relative error of the tcgen05 Gram
+// would move the sweep at which the coordinate descent stops), the coordinate descent (enet.cuh), then the model
+// X[:, :-1] w[:-1] minus its median over all cadences (rg_final on the coefficients with the last one zeroed).
+int elasticnet(const double* X, int x_batched, const double* y, const uint8_t* cadence_mask, int B, int64_t N, int K,
+               double alpha, double l1_ratio, int max_iter, double tol, int positive, double* coeff, double* model,
+               int32_t* n_iter, double* dual_gap, uint8_t* converged, int mem, cudaStream_t st) {
+  LKB_REQUIRE(X && y && coeff && model && n_iter && dual_gap && converged, "lkb_elasticnet: null argument");
+  LKB_REQUIRE(B > 0 && B <= 65535 && N > 0 && K > 0, "lkb_elasticnet: bad sizes");
+  LKB_REQUIRE(N < ((int64_t)1 << 31), "lkb_elasticnet: N too large");
+  if (!(alpha >= 0.0) || !std::isfinite(alpha)) { set_error("lkb_elasticnet: alpha must be >= 0 (got %g)", alpha); return LKB_E_ARG; }
+  if (!(l1_ratio >= 0.0 && l1_ratio <= 1.0)) {
+    set_error("lkb_elasticnet: l1_ratio must be in [0, 1] (got %g)", l1_ratio);
+    return LKB_E_ARG;
+  }
+  if (max_iter < 1) { set_error("lkb_elasticnet: max_iter must be >= 1 (got %d)", max_iter); return LKB_E_ARG; }
+  if (!(tol >= 0.0)) { set_error("lkb_elasticnet: tol must be >= 0 (got %g)", tol); return LKB_E_ARG; }
+  if (K > ENET_KMAX) { set_error("lkb_elasticnet: K=%d > %d unsupported", K, ENET_KMAX); return LKB_E_UNSUPPORTED; }
+  LKB_TRY(ensure_device());
+  const int Ka = K + 1;
+  const size_t BN = (size_t)B * N;
+
+  const double *d_X = nullptr, *d_y = nullptr;
+  const uint8_t* d_cm = nullptr;
+  LKB_TRY(stage_in<double>(mem, WS_IN0, X, (x_batched ? BN : (size_t)N) * K, &d_X, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN1, y, BN, &d_y, st));
+  LKB_TRY(stage_in<uint8_t>(mem, WS_IN3, cadence_mask, BN, &d_cm, st));
+
+  RgWs ws{};
+  uint8_t* d_none = nullptr;                           // the (empty) outlier mask rg_rows reads
+  double* d_w0 = nullptr;                              // coefficients with the constant's entry zeroed, for the model
+  LKB_TRY(ws_get_t<int32_t>(WS_A, BN, &ws.rows));
+  LKB_TRY(ws_get_t<int32_t>(WS_B, B, &ws.cnt));
+  LKB_TRY(ws_get_t<uint8_t>(WS_C, BN, &ws.used));
+  LKB_TRY(ws_get_t<double>(WS_D, (size_t)B * Ka * Ka, &ws.gram));
+  LKB_TRY(ws_get_t<double>(WS_H, BN, &ws.wl));
+  LKB_TRY(ws_get_t<uint8_t>(WS_E, BN, &d_none));
+  LKB_TRY(ws_get_t<double>(WS_F, (size_t)B * K, &d_w0));
+
+  double *o_c = nullptr, *o_m = nullptr, *o_g = nullptr;
+  int32_t* o_it = nullptr;
+  uint8_t* o_cv = nullptr;
+  LKB_TRY(stage_out_alloc<double>(mem, WS_OUT0, coeff, (size_t)B * K, &o_c));
+  LKB_TRY(stage_out_alloc<double>(mem, WS_OUT1, model, BN, &o_m));
+  LKB_TRY(stage_out_alloc<int32_t>(mem, WS_OUT2, n_iter, B, &o_it));
+  LKB_TRY(stage_out_alloc<double>(mem, WS_OUT3, dual_gap, B, &o_g));
+  LKB_TRY(stage_out_alloc<uint8_t>(mem, WS_OUT4, converged, B, &o_cv));
+
+  {
+    const int64_t ng = (int64_t)B * Ka * Ka, nz = ng > (int64_t)BN ? ng : (int64_t)BN;
+    rg_zero_kernel<<<(unsigned)((nz + 255) / 256), 256, 0, st>>>(ws.gram, ng, d_none, (int64_t)BN);
+    LKB_LAUNCH_CHECK();
+  }
+  rg_rows_kernel<<<B, 256, 0, st>>>(d_cm, d_none, nullptr, N, 1, ws);
+  LKB_LAUNCH_CHECK();
+  {
+    // a light curve without a used cadence has no fit (scikit-learn refuses an empty X)
+    int32_t* h_cnt = (int32_t*)malloc(sizeof(int32_t) * (size_t)B);
+    if (!h_cnt) { set_error("lkb_elasticnet: host allocation failed"); return LKB_E_OOM; }
+    cudaError_t e = cudaMemcpyAsync(h_cnt, ws.cnt, sizeof(int32_t) * (size_t)B, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    int empty = -1;
+    for (int b = 0; b < B && e == cudaSuccess; ++b)
+      if (h_cnt[b] == 0) { empty = b; break; }
+    free(h_cnt);
+    LKB_CUDA_CHECK(e);
+    if (empty >= 0) {
+      set_error("lkb_elasticnet: light curve %d has no used cadence", empty);
+      return LKB_E_ARG;
+    }
+  }
+  prof_begin(st);
+  LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, nullptr, B, N, K, 1.0, true, ws, st));
+  LKB_LAUNCH_CHECK();
+  prof_end(st);
+  prof_begin(st);
+  LKB_TRY(enet_cd_launch(ws.gram, ws.cnt, B, K, alpha, l1_ratio, max_iter, tol, positive, o_c, o_it, o_g, o_cv, st));
+  prof_end(st);
+  prof_begin(st);
+  LKB_CUDA_CHECK(cudaMemcpyAsync(d_w0, o_c, sizeof(double) * (size_t)B * K, cudaMemcpyDeviceToDevice, st));
+  LKB_CUDA_CHECK(cudaMemset2DAsync(d_w0 + (K - 1), sizeof(double) * K, 0, sizeof(double), B, st));
+  rg_final_kernel<<<B, 512, K * sizeof(double), st>>>(d_X, x_batched, N, K, d_w0, o_m, 0);
+  LKB_LAUNCH_CHECK();
+  prof_end(st);
+
+  LKB_TRY(stage_out_copy<double>(mem, coeff, o_c, (size_t)B * K, st));
+  LKB_TRY(stage_out_copy<double>(mem, model, o_m, BN, st));
+  LKB_TRY(stage_out_copy<int32_t>(mem, n_iter, o_it, B, st));
+  LKB_TRY(stage_out_copy<double>(mem, dual_gap, o_g, B, st));
+  LKB_TRY(stage_out_copy<uint8_t>(mem, converged, o_cv, B, st));
   if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
   return LKB_OK;
 }

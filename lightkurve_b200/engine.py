@@ -428,6 +428,32 @@ def regress(X, Y, flux_err=None, cadence_mask=None, prior_mu=None, prior_sigma=N
     return out
 
 
+def elasticnet(X, Y, cadence_mask=None, alpha=1e-20, l1_ratio=0.01, max_iter=1000, tol=1e-4, positive=False):
+    """K8.  scikit-learn's ElasticNet(alpha, l1_ratio, fit_intercept=False, max_iter, tol, positive).fit on the used
+    cadences of each light curve, and the CBVCorrector model.  X [N, K] (shared) or [B, N, K]; Y [B, N]; cadence_mask
+    bool [B, N] or None (all).  Returns dict(coefficients [B, K], model [B, N] (= X[:, :-1] coef[:-1] minus its
+    median over all cadences), n_iter int32 [B], dual_gap [B], converged bool [B])."""
+    lib = L.load()
+    X = np.ascontiguousarray(X, dtype=np.float64)
+    Y = np.ascontiguousarray(np.atleast_2d(Y), dtype=np.float64)
+    B, N = Y.shape
+    batched = X.ndim == 3
+    K = X.shape[-1]
+    if X.ndim not in (2, 3) or X.shape[-2] != N or (batched and X.shape[0] != B):
+        raise ValueError("X shape %s does not match Y shape %s" % (X.shape, Y.shape))
+    cm = None if cadence_mask is None else \
+        np.ascontiguousarray(np.broadcast_to(np.asarray(cadence_mask, dtype=bool), Y.shape).astype(np.uint8))
+    coeff = np.empty((B, K), dtype=np.float64)
+    model = np.empty((B, N), dtype=np.float64)
+    n_iter = np.empty(B, dtype=np.int32)
+    gap = np.empty(B, dtype=np.float64)
+    conv = np.empty(B, dtype=np.uint8)
+    L.check(lib.lkb_elasticnet(L.ptr(X), 1 if batched else 0, L.ptr(Y), L.ptr(cm), B, N, K, float(alpha),
+                               float(l1_ratio), int(max_iter), float(tol), 1 if positive else 0, L.ptr(coeff),
+                               L.ptr(model), L.ptr(n_iter), L.ptr(gap), L.ptr(conv), L.MEM_HOST, None))
+    return dict(coefficients=coeff, model=model, n_iter=n_iter, dual_gap=gap, converged=conv.astype(bool))
+
+
 def nanmedian_std(arrays):
     """K6.  np.nanmedian and np.nanstd of each array."""
     lib = L.load()
