@@ -274,7 +274,9 @@ __device__ double block_nanmedian_fast(Get get, int64_t n, SelSmem& sm, FastSelS
         continue;
       }
     }
-    if (observed) *observed = true;                              // every element went past obs exactly once
+    // every element went past obs exactly once; but a fresh sample's bracket may miss above the median (lo > median:
+    // more than klo values below lo), and then obs was not given a lower bound of the median
+    if (observed) *observed = m > 0 && klo >= t_lt;
     if (br && threadIdx.x == 0) { br->lo = lo; br->hi = hi; br->valid = n_cand <= FS_CAP; }   // (barriers follow)
     if (n_cand > FS_CAP) return block_nanmedian(get, n, sm);
     auto getc = [&](int64_t i) { return fs.cand[i]; };

@@ -61,3 +61,25 @@ def test_bls_matches_astropy_bit_exact_bins():
     for k, rk in (("power", "power"), ("depth", "depth"), ("depth_err", "depth_err"), ("duration", "duration"),
                   ("transit_time", "transit_time"), ("depth_snr", "depth_snr"), ("log_likelihood", "log_likelihood")):
         np.testing.assert_allclose(got[k], np.asarray(getattr(ref, rk)), rtol=1e-12, atol=1e-14, err_msg=k)
+
+
+@pytest.mark.parametrize("case", ["normal_flares", "deep_dips"])
+def test_sigma_clip_mask_matches_astropy(case):
+    """oracle.detrend.sigma_clip_mask (and rg_clip_kernel, which tests/test_regress_clip_emulated.py pins to it) keeps
+    a value masked once a round has clipped it.  If astropy's final mask were instead "outside the LAST round's
+    bounds", the two would differ where a value clipped early lies inside the final bounds: one-sided deep dips move
+    the median between rounds, which is where that shows."""
+    from astropy.stats import sigma_clip
+
+    from oracle import detrend as odet
+    rng = np.random.default_rng(11)
+    x = rng.normal(size=20000)
+    if case == "normal_flares":
+        x[rng.choice(20000, 200, replace=False)] += rng.exponential(6.0, 200)
+    else:
+        for s in rng.choice(19960, 60, replace=False):
+            x[s:s + 30] -= np.exp(rng.uniform(np.log(2.0), np.log(80.0)))
+    x[::997] = np.nan
+    for sigma in (3.0, 5.0):
+        ref = np.ma.getmaskarray(sigma_clip(x, sigma=sigma, maxiters=5))
+        np.testing.assert_array_equal(odet.sigma_clip_mask(x, sigma), ref)
