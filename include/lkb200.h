@@ -162,6 +162,17 @@ int lkb_bls_power(const double* t, const double* y, const double* dy, const int6
                   double* power, double* depth, double* depth_err, double* duration_out,
                   double* transit_time, double* depth_snr, double* log_likelihood,
                   int32_t* best_bins, int mem, void* stream);
+/* The same for light curves with their own period grids (lkb_bls_power is this call with period_offsets == NULL):
+ *   period_offsets == NULL: one grid of P periods shared by all light curves; outputs [B,P].
+ *   else: host CSR int64 [B+1] into `period` (period_offsets[0] == 0, period_offsets[B] == P, no light curve with
+ *         an empty grid); every output (and best_bins, 2 entries per period) uses the same CSR layout.
+ * Each light curve's result is bitwise the result of a one-light-curve lkb_bls_power call on its own grid. */
+int lkb_bls_power_ex(const double* t, const double* y, const double* dy, const int64_t* offsets, int B,
+                     const double* period, const int64_t* period_offsets, int64_t P,
+                     const double* duration, int D, int oversample, int objective,
+                     double* power, double* depth, double* depth_err, double* duration_out,
+                     double* transit_time, double* depth_snr, double* log_likelihood,
+                     int32_t* best_bins, int mem, void* stream);
 
 /* Debug/parity entry: the per-sample bin index of bls.c for ONE period,
  * ind[n] = (int)(fabs(fmod(t[n]-min_t, period))/bin_duration)+1, evaluated by the

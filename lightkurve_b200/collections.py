@@ -66,15 +66,18 @@ class LightCurveCollection(Collection):
         if len(self.data) == 0:
             return []
         if method in ("bls", "boxleastsquares"):
+            # one engine call: the shared-grid entry when every light curve has the same grid, else per-light-curve
+            # grids; light curves without usable flux_err get unit weights (bitwise the weights of dy=None)
             preps = [BoxLeastSquaresPeriodogram._prepare(lc, **dict(kwargs)) for lc in self.data]
             p0 = preps[0]
-            same = all(np.array_equal(p["period"], p0["period"]) and np.array_equal(p["duration"], p0["duration"])
-                       and (p["dy"] is None) == (p0["dy"] is None) for p in preps)
-            if not same:
-                return [lc.to_periodogram(method, **dict(kwargs)) for lc in self.data]
-            res = engine.bls_power([p["time"] for p in preps], [p["flux"] for p in preps],
-                                   None if p0["dy"] is None else [p["dy"] for p in preps], p0["period"],
-                                   p0["duration"], oversample=p0["oversample"], objective=p0["objective"])
+            same = all(len(p["period"]) == len(p0["period"]) and np.array_equal(p["period"], p0["period"])
+                       for p in preps)
+            dys = None
+            if any(p["dy"] is not None for p in preps):
+                dys = [np.ones(len(p["time"])) if p["dy"] is None else p["dy"] for p in preps]
+            res = engine.bls_power([p["time"] for p in preps], [p["flux"] for p in preps], dys,
+                                   p0["period"] if same else [p["period"] for p in preps], p0["duration"],
+                                   oversample=p0["oversample"], objective=p0["objective"])
             out = []
             for b, p in enumerate(preps):
                 pg = BoxLeastSquaresPeriodogram._finish(p, res, b)

@@ -212,9 +212,9 @@ int ls_power_shared(const double*, const void*, int, int, int64_t, const double*
                     float*, int, cudaStream_t, int);
 int ls_power_chi2(const double*, const void*, int, const int64_t*, int, const double*, const int64_t*, int64_t, int,
                   int, const double*, float*, double*, int, cudaStream_t, int);
-int bls_power(const double*, const double*, const double*, const int64_t*, int, const double*, int64_t,
-              const double*, int, int, int, double*, double*, double*, double*, double*, double*, double*, int32_t*,
-              int, cudaStream_t);
+int bls_power(const double*, const double*, const double*, const int64_t*, int, const double*, const int64_t*,
+              int64_t, const double*, int, int, int, double*, double*, double*, double*, double*, double*, double*,
+              int32_t*, int, cudaStream_t);
 int bls_bin_index(const double*, int64_t, double, double, double, int32_t*, int, cudaStream_t);
 int flatten(const double*, const double*, const double*, const uint8_t*, const int64_t*, int, int, int, double, int,
             double, double*, double*, double*, int, cudaStream_t);
@@ -360,9 +360,19 @@ int lkb_bls_power(const double* t, const double* y, const double* dy, const int6
                   const double* period, int64_t P, const double* duration, int D, int oversample, int objective,
                   double* power, double* depth, double* depth_err, double* duration_out, double* transit_time,
                   double* depth_snr, double* log_likelihood, int32_t* best_bins, int mem, void* stream) {
+  return lkb_bls_power_ex(t, y, dy, offsets, B, period, nullptr, P, duration, D, oversample, objective, power, depth,
+                          depth_err, duration_out, transit_time, depth_snr, log_likelihood, best_bins, mem, stream);
+}
+
+int lkb_bls_power_ex(const double* t, const double* y, const double* dy, const int64_t* offsets, int B,
+                     const double* period, const int64_t* period_offsets, int64_t P, const double* duration, int D,
+                     int oversample, int objective, double* power, double* depth, double* depth_err,
+                     double* duration_out, double* transit_time, double* depth_snr, double* log_likelihood,
+                     int32_t* best_bins, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  return bls_power(t, y, dy, offsets, B, period, P, duration, D, oversample, objective, power, depth, depth_err,
-                   duration_out, transit_time, depth_snr, log_likelihood, best_bins, mem, (cudaStream_t)stream);
+  return bls_power(t, y, dy, offsets, B, period, period_offsets, P, duration, D, oversample, objective, power, depth,
+                   depth_err, duration_out, transit_time, depth_snr, log_likelihood, best_bins, mem,
+                   (cudaStream_t)stream);
 }
 
 int lkb_bls_bin_index(const double* t_rel, int64_t N, double min_t, double period, double bin_duration,

@@ -27,14 +27,12 @@
 // scan construction (see bls_cumsum).
 #include "common.cuh"
 #include "select.cuh"
+#include "bls_plan.h"
 #include <float.h>
 #include <algorithm>
 #include <vector>
 
 namespace lkb {
-
-constexpr int BLS_WARPS = 8;
-constexpr int BLS_TILE = 1024;
 
 // exact fmod for finite x, p != 0, |x/p| < 2^50 (true for any real light curve)
 __device__ __forceinline__ double bls_fmod(double x, double p, double inv_p) {
@@ -197,8 +195,8 @@ bls_prep_kernel(const double* __restrict__ t, const double* __restrict__ y, cons
 // T[j] = first cadence with x >= j * delta (lower bound), j = 0 .. nT - 1, per light curve.
 __global__ void __launch_bounds__(256)
 bls_table_kernel(const double* __restrict__ trel, const int64_t* __restrict__ offsets,
-                 const int64_t* __restrict__ tab_offsets, double delta, int32_t* __restrict__ tab) {
-  const int b = blockIdx.y;
+                 const int64_t* __restrict__ tab_offsets, int b_base, double delta, int32_t* __restrict__ tab) {
+  const int b = b_base + blockIdx.y;           // the launch covers light curves [b_base, b_base + gridDim.y)
   const int64_t o = offsets[b], n = offsets[b + 1] - o;
   const int64_t to = tab_offsets[b], nT = tab_offsets[b + 1] - to;
   const double* x = trel + o;
@@ -359,7 +357,7 @@ __device__ __forceinline__ void bls_finish_warp(double2* h, int n_bins, int over
 struct BlsFast {            // boundary-path inputs (null tab => cadence path only)
   const double2* cpre;      // [total + B] exclusive prefix sums
   const int32_t* tab;       // lookup tables
-  const int64_t* tab_offsets;
+  const int64_t* tab_offsets;  // [b] .. [b + 1]: light curve b's table (b in the current table group)
   double delta, inv_delta;
   double min_density;       // use the boundary path when N >= min_density * (x_max / bin_duration)
 };
@@ -369,9 +367,9 @@ template <bool GHIST>
 __global__ void __launch_bounds__(BLS_WARPS * 32)
 bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy, const double* __restrict__ iv,
                   const int64_t* __restrict__ offsets, const BlsLcInfo* __restrict__ info,
-                  const double* __restrict__ period, int64_t p_begin, int64_t p_end, int64_t P,
+                  const double* __restrict__ period, const BlsCta* __restrict__ cta, int64_t out_stride,
                   const int* __restrict__ dur_bins, int D, double bin_duration,
-                  int oversample, int objective, int hist_stride, double2* __restrict__ g_hist, BlsFast fast, int b_base,
+                  int oversample, int objective, int hist_stride, double2* __restrict__ g_hist, BlsFast fast,
                   double* __restrict__ o_power, double* __restrict__ o_depth, double* __restrict__ o_depth_err,
                   double* __restrict__ o_duration, double* __restrict__ o_ttime, double* __restrict__ o_snr,
                   double* __restrict__ o_ll, int32_t* __restrict__ o_bins) {
@@ -382,21 +380,22 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
   double2* s_hist = s_scr + BLS_WARPS * 32;                       // BLS_WARPS * hist_stride (unless GHIST)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = b_base + blockIdx.y;            // the launch covers light curves [b_base, b_base + gridDim.y)
+  const BlsCta d = cta[blockIdx.x];             // this CTA: periods d.p .. d.p + d.n - 1 of light curve d.b
+  const int b = d.b;
   const int64_t o = offsets[b], n = offsets[b + 1] - o;
   const int nwarps = blockDim.x >> 5;
-  const int64_t p = p_begin + (int64_t)blockIdx.x * nwarps + warp;
+  const int p = d.p + warp;                     // index into `period` (< 2^31); output at b * out_stride + p
   if (n <= 0) {      // empty light curve: every output NaN
-    if (p < p_end && lane == 0) {
+    if (warp < d.n && lane == 0) {
       const double qn = __longlong_as_double(0x7ff8000000000000ll);
-      const int64_t oi = (int64_t)b * P + p;
+      const int64_t oi = (int64_t)b * out_stride + p;
       o_power[oi] = qn; o_depth[oi] = qn; o_depth_err[oi] = qn; o_duration[oi] = qn; o_ttime[oi] = qn;
       o_snr[oi] = qn; o_ll[oi] = qn;
       if (o_bins) { o_bins[2 * oi] = -1; o_bins[2 * oi + 1] = -1; }
     }
     return;
   }
-  const bool active = p < p_end;
+  const bool active = warp < d.n;
   const double per = active ? period[p] : 1.0;
   const double inv_per = 1.0 / per;
   const double inv_bin = 1.0 / bin_duration;
@@ -407,7 +406,7 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
 
   double2* h;
   if constexpr (GHIST) {
-    const size_t slot = ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * nwarps + warp;
+    const size_t slot = (size_t)blockIdx.x * nwarps + warp;
     h = g_hist + slot * (size_t)hist_stride;
   } else {
     h = s_hist + (size_t)warp * hist_stride;
@@ -521,7 +520,7 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
   }
   __syncwarp();
   bls_finish_warp(h, n_bins, oversample, s_scr + warp * 32, lane, li, dur_bins, D, bin_duration, objective, per,
-                  inv_per, (int64_t)b * P + p, o_power, o_depth, o_depth_err, o_duration, o_ttime, o_snr, o_ll, o_bins);
+                  inv_per, (int64_t)b * out_stride + p, o_power, o_depth, o_depth_err, o_duration, o_ttime, o_snr, o_ll, o_bins);
 }
 
 // ---- host ------------------------------------------------------------------------------------
@@ -542,14 +541,24 @@ int bls_bin_index(const double* t_rel, int64_t N, double min_t, double period, d
 }
 
 int bls_power(const double* t, const double* y, const double* dy, const int64_t* h_offsets, int B,
-              const double* period, int64_t P, const double* duration, int D, int oversample, int objective,
-              double* power, double* depth, double* depth_err, double* duration_out, double* transit_time,
-              double* depth_snr, double* log_like, int32_t* best_bins, int mem, cudaStream_t st) {
+              const double* period, const int64_t* period_offsets, int64_t P, const double* duration, int D,
+              int oversample, int objective, double* power, double* depth, double* depth_err, double* duration_out,
+              double* transit_time, double* depth_snr, double* log_like, int32_t* best_bins, int mem,
+              cudaStream_t st) {
   LKB_REQUIRE(t && y && h_offsets && period && duration, "lkb_bls_power: null input");
   LKB_REQUIRE(power && depth && depth_err && duration_out && transit_time && depth_snr && log_like,
               "lkb_bls_power: null output");
   LKB_REQUIRE(B > 0 && B <= 65535 && P > 0 && D > 0 && oversample > 0, "lkb_bls_power: bad sizes");
   LKB_REQUIRE(objective == 0 || objective == 1, "lkb_bls_power: bad objective");
+  LKB_REQUIRE(P < ((int64_t)1 << 31), "lkb_bls_power: more than 2^31 - 1 periods");
+  const int64_t* pofs = period_offsets;
+  if (pofs) {
+    LKB_REQUIRE(pofs[0] == 0 && pofs[B] == P, "lkb_bls_power: period_offsets[0] must be 0 and period_offsets[B] == P");
+    for (int b = 0; b < B; ++b) {
+      if (pofs[b + 1] < pofs[b]) { set_error("lkb_bls_power: period_offsets decrease at light curve %d", b); return LKB_E_ARG; }
+      if (pofs[b + 1] == pofs[b]) { set_error("lkb_bls_power: light curve %d has an empty period grid", b); return LKB_E_ARG; }
+    }
+  }
   LKB_TRY(ensure_device());
   const int64_t total = h_offsets[B];
 
@@ -563,21 +572,38 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
     LKB_CUDA_CHECK(cudaMemcpyAsync(h_dur.data(), duration, sizeof(double) * D, cudaMemcpyDeviceToHost, st));
     LKB_CUDA_CHECK(cudaStreamSynchronize(st));
   }
-  double min_period = h_per[0], max_period = h_per[0], min_dur = h_dur[0], max_dur = h_dur[0];
-  for (int64_t i = 0; i < P; ++i) {
-    if (!(h_per[i] == h_per[i]) || isinf(h_per[i])) { set_error("lkb_bls_power: period contains nan/inf"); return LKB_E_ARG; }
-    min_period = fmin(min_period, h_per[i]);
-    max_period = fmax(max_period, h_per[i]);
+  // per grid (the shared one, or each light curve's own): finite periods, and its minimum
+  const int n_grids = pofs ? B : 1;
+  std::vector<double> grid_min(n_grids);
+  for (int g = 0; g < n_grids; ++g) {
+    const int64_t q0 = pofs ? pofs[g] : 0, q1 = pofs ? pofs[g + 1] : P;
+    double mn = h_per[q0];
+    for (int64_t i = q0; i < q1; ++i) {
+      if (!(h_per[i] == h_per[i]) || isinf(h_per[i])) {
+        if (pofs) set_error("lkb_bls_power: period of light curve %d contains nan/inf", g);
+        else set_error("lkb_bls_power: period contains nan/inf");
+        return LKB_E_ARG;
+      }
+      mn = fmin(mn, h_per[i]);
+    }
+    grid_min[g] = mn;
   }
+  double min_dur = h_dur[0], max_dur = h_dur[0];
   for (int i = 0; i < D; ++i) {
     if (!(h_dur[i] == h_dur[i]) || isinf(h_dur[i])) { set_error("lkb_bls_power: duration contains nan/inf"); return LKB_E_ARG; }
     min_dur = fmin(min_dur, h_dur[i]);
     max_dur = fmax(max_dur, h_dur[i]);
   }
-  if (min_period < DBL_EPSILON) { set_error("lkb_bls_power: periods must be positive"); return LKB_E_ARG; }
-  if (max_dur >= min_period || min_dur < DBL_EPSILON) {
-    set_error("The maximum transit duration must be shorter than the minimum period");
-    return LKB_E_ARG;
+  for (int g = 0; g < n_grids; ++g) {
+    if (grid_min[g] < DBL_EPSILON) {
+      if (pofs) set_error("lkb_bls_power: periods of light curve %d must be positive", g);
+      else set_error("lkb_bls_power: periods must be positive");
+      return LKB_E_ARG;
+    }
+    if (max_dur >= grid_min[g] || min_dur < DBL_EPSILON) {
+      set_error("The maximum transit duration must be shorter than the minimum period");
+      return LKB_E_ARG;
+    }
   }
   const double bin_duration = min_dur / (double)oversample;
   std::vector<int> h_durbins(D);
@@ -604,7 +630,9 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
   LKB_TRY(ws_get_t<double>(WS_E, total, &d_iv));
   LKB_TRY(ws_get_t<BlsLcInfo>(WS_F, B, &d_info));
 
-  const size_t outn = (size_t)B * P;
+  // outputs: [B, P] for a shared grid, the CSR layout of `period` for per-light-curve grids
+  const size_t outn = pofs ? (size_t)P : (size_t)B * P;
+  const int64_t out_stride = pofs ? 0 : P;
   double *o0, *o1, *o2, *o3, *o4, *o5, *o6;
   int32_t* ob = nullptr;
   LKB_TRY(stage_out_alloc<double>(mem, WS_OUT0, power, outn, &o0));
@@ -621,7 +649,8 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
   bls_prep_kernel<<<B, 256, 0, st>>>(d_t, d_y, d_dy, d_off, d_trel, d_wy, d_iv, d_cpre, d_info);
   LKB_LAUNCH_CHECK();
 
-  // boundary path set-up: per-light-curve lookup tables "first cadence at or after j * delta"
+  // boundary path set-up: per-light-curve lookup tables "first cadence at or after j * delta", built per table
+  // group (bls_plan.h) just before that group's search
   BlsFast fast;
   fast.cpre = d_cpre;
   fast.tab = nullptr;
@@ -630,101 +659,99 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
   fast.inv_delta = 1.0 / fast.delta;
   fast.min_density = 0.8;
   if (const char* e = getenv("LKB_BLS_MIN_DENSITY")) fast.min_density = atof(e);
+  std::vector<int64_t> h_to;
+  std::vector<BlsTableGroup> groups;
   {
     std::vector<BlsLcInfo> h_info(B);
     LKB_CUDA_CHECK(cudaMemcpyAsync(h_info.data(), d_info, sizeof(BlsLcInfo) * B, cudaMemcpyDeviceToHost, st));
     LKB_CUDA_CHECK(cudaStreamSynchronize(st));
-    std::vector<int64_t> h_to(B + 1, 0);
-    bool ok = fast.min_density < 1e30;
-    int64_t nT_max = 0;
-    for (int b = 0; b < B && ok; ++b) {
-      const int64_t nb = h_offsets[b + 1] - h_offsets[b];
-      int64_t nT = 0;
-      if (nb > 0) {
-        const double cells = h_info[b].x_max * fast.inv_delta;
-        if (!(cells >= 0.0) || cells > 6.0e7) { ok = false; break; }
-        nT = (int64_t)cells + 3;
-      }
-      h_to[b + 1] = h_to[b] + nT;
-      nT_max = nT > nT_max ? nT : nT_max;
+    std::vector<int64_t> n(B);
+    std::vector<double> x_max(B);
+    for (int b = 0; b < B; ++b) {
+      n[b] = h_offsets[b + 1] - h_offsets[b];
+      x_max[b] = h_info[b].x_max;
     }
-    if (ok && h_to[B] > 0 && h_to[B] <= ((int64_t)1 << 28)) {
-      int64_t* d_to = nullptr;
-      int32_t* d_tab = nullptr;
-      LKB_TRY(ws_get_t<int64_t>(WS_I, B + 1, &d_to));
-      LKB_TRY(ws_get_t<int32_t>(WS_J, h_to[B], &d_tab));
-      LKB_CUDA_CHECK(cudaMemcpyAsync(d_to, h_to.data(), sizeof(int64_t) * (B + 1), cudaMemcpyHostToDevice, st));
-      LKB_CUDA_CHECK(cudaStreamSynchronize(st));   // h_to is a local
-      const unsigned gxT = (unsigned)min((int64_t)64, (nT_max + 255) / 256);
-      bls_table_kernel<<<dim3(gxT ? gxT : 1, (unsigned)B), 256, 0, st>>>(d_trel, d_off, d_to, fast.delta, d_tab);
-      LKB_LAUNCH_CHECK();
-      fast.tab = d_tab;
-      fast.tab_offsets = d_to;
-    }
+    groups = bls_table_groups(n.data(), x_max.data(), B, fast.inv_delta, fast.min_density < 1e30, pofs == nullptr,
+                              BLS_TABLE_BUDGET, h_to);
   }
+  // search launches: CTA descriptors of every table group, uploaded once
+  BlsPlanLimits lim;
+  static const int ghist_bins = getenv("LKB_BLS_GHIST_BINS") ? atoi(getenv("LKB_BLS_GHIST_BINS")) : -1;
+  lim.ghist_bins = ghist_bins;
+  if (getenv("LKB_BLS_HIST_CAP_MB")) lim.hist_cap = (size_t)atoll(getenv("LKB_BLS_HIST_CAP_MB")) << 20;
+  BlsPlan plan;
+  std::vector<size_t> group_launch(groups.size() + 1, 0);
+  for (size_t gi = 0; gi < groups.size(); ++gi) {
+    char msg[256];
+    if (!bls_plan(h_per.data(), pofs, P, groups[gi].b0, groups[gi].b1, bin_duration, oversample, lim, plan, msg,
+                  sizeof msg)) {
+      set_error("%s", msg);
+      return LKB_E_UNSUPPORTED;
+    }
+    group_launch[gi + 1] = plan.launch.size();
+  }
+  int64_t tab_max = 0;
+  for (const BlsTableGroup& g : groups)
+    if (g.table) tab_max = std::max(tab_max, h_to[g.b1] - h_to[g.b0]);
+  // table offsets relative to each group's first entry: group g's light curves b0 .. b1 (inclusive) at [b + g]
+  std::vector<int64_t> h_torel(B + groups.size());
+  for (size_t gi = 0; gi < groups.size(); ++gi)
+    for (int b = groups[gi].b0; b <= groups[gi].b1; ++b) h_torel[b + gi] = h_to[b] - h_to[groups[gi].b0];
+  int64_t* d_to = nullptr;
+  int32_t* d_tab = nullptr;
+  if (tab_max > 0) {
+    LKB_TRY(ws_get_t<int64_t>(WS_I, h_torel.size(), &d_to));
+    LKB_TRY(ws_get_t<int32_t>(WS_J, tab_max, &d_tab));
+    LKB_CUDA_CHECK(cudaMemcpyAsync(d_to, h_torel.data(), sizeof(int64_t) * h_torel.size(), cudaMemcpyHostToDevice, st));
+  }
+  BlsCta* d_cta = nullptr;
+  LKB_TRY(ws_get_t<BlsCta>(WS_K, plan.cta.size(), &d_cta));
+  LKB_CUDA_CHECK(cudaMemcpyAsync(d_cta, plan.cta.data(), sizeof(BlsCta) * plan.cta.size(), cudaMemcpyHostToDevice, st));
+  double2* g_hist = nullptr;
+  if (plan.ghist_bytes > 0) LKB_TRY(ws_get_t<double2>(WS_G, plan.ghist_bytes / sizeof(double2), &g_hist));
+  LKB_CUDA_CHECK(cudaStreamSynchronize(st));   // h_torel and plan.cta are locals
 
-  // chunk the period list so that one launch's per-warp histograms have a common size
-  const size_t fixed_smem = (size_t)(3 * BLS_TILE + 2 + 2 * BLS_WARPS * 32) * sizeof(double);
-  const size_t smem_cap = 200 * 1024;
   static bool attr_set = false;
   if (!attr_set) {
     LKB_CUDA_CHECK(cudaFuncSetAttribute(bls_search_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     LKB_CUDA_CHECK(cudaFuncSetAttribute(bls_search_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  int64_t p0 = 0;
+  auto launch_tables = [&](size_t gi) {
+    const BlsTableGroup& g = groups[gi];
+    if (!g.table) {
+      fast.tab = nullptr;
+      fast.tab_offsets = nullptr;
+      return;
+    }
+    int64_t nT_max = 0;
+    for (int b = g.b0; b < g.b1; ++b) nT_max = std::max(nT_max, h_to[b + 1] - h_to[b]);
+    const unsigned gxT = (unsigned)min((int64_t)64, (nT_max + 255) / 256);
+    bls_table_kernel<<<dim3(gxT ? gxT : 1, (unsigned)(g.b1 - g.b0)), 256, 0, st>>>(d_trel, d_off, d_to + gi, g.b0,
+                                                                                   fast.delta, d_tab);
+    fast.tab = d_tab;
+    fast.tab_offsets = d_to + gi;
+  };
+  launch_tables(0);
+  LKB_LAUNCH_CHECK();
   prof_begin(st);
-  while (p0 < P) {
-    int nb_min = (int)ceil(h_per[p0] / bin_duration) + oversample, nb_max = nb_min;
-    int64_t p1 = p0 + 1;
-    while (p1 < P) {
-      const int nb = (int)ceil(h_per[p1] / bin_duration) + oversample;
-      const int lo = nb < nb_min ? nb : nb_min, hi = nb > nb_max ? nb : nb_max;
-      if (hi > lo + lo / 4 + 64) break;
-      nb_min = lo; nb_max = hi;
-      ++p1;
-    }
-    const int stride = ((nb_max + 1 + 3) / 4) * 4;
-    // warps (= periods) per CTA: as many as fit with their private histograms in shared memory
-    int W = BLS_WARPS;
-    while (W > 1 && fixed_smem + (size_t)W * 2 * stride * sizeof(double) > smem_cap) W >>= 1;
-    size_t hist_bytes = (size_t)W * 2 * stride * sizeof(double);
-    double2* g_hist = nullptr;
-    size_t smem = fixed_smem + hist_bytes;
-    // Occupancy beats locality here (measured: 108 -> 84 ms on the config-3 probe): once the shared-memory
-    // histograms would leave fewer than 4 CTAs (32 warps) per SM, keep them in the L2-resident workspace.
-    static const int ghist_bins = getenv("LKB_BLS_GHIST_BINS") ? atoi(getenv("LKB_BLS_GHIST_BINS")) : -1;
-    if (ghist_bins >= 0 ? stride > ghist_bins : 4 * (smem + 1024) > 227 * 1024) smem = smem_cap + 1;
-    if (smem > smem_cap) { W = BLS_WARPS; hist_bytes = (size_t)W * 2 * stride * sizeof(double); }
-    const unsigned gx = (unsigned)((p1 - p0 + W - 1) / W);
-    int b_group = B;
-    if (smem > smem_cap) {
-      // histograms do not fit in shared memory: keep them in (L2-resident) global workspace
-      smem = fixed_smem;
-      // one histogram slot per warp of the launch: bound the workspace by launching the light curves in groups
-      const size_t per_lc = (size_t)gx * hist_bytes;
-      const size_t cap = getenv("LKB_BLS_HIST_CAP_MB") ? (size_t)atoll(getenv("LKB_BLS_HIST_CAP_MB")) << 20 : (size_t)12 << 30;
-      if (per_lc > cap) {
-        set_error("lkb_bls_power: %d bins per period needs %zu bytes of histogram workspace per light curve", nb_max,
-                  per_lc);
-        return LKB_E_UNSUPPORTED;
-      }
-      b_group = (int)std::min<size_t>((size_t)B, std::max<size_t>(1, cap / per_lc));
-      LKB_TRY(ws_get_t<double2>(WS_G, per_lc * b_group / sizeof(double2), &g_hist));
-    }
-    for (int bb = 0; bb < B; bb += b_group) {
-      dim3 grid(gx, (unsigned)std::min(b_group, B - bb));
-      if (g_hist)
-        bls_search_kernel<true><<<grid, W * 32, smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per, p0, p1, P,
-                                                            d_durbins, D, bin_duration, oversample, objective, stride,
-                                                            g_hist, fast, bb, o0, o1, o2, o3, o4, o5, o6, ob);
+  for (size_t gi = 0; gi < groups.size(); ++gi) {
+    if (gi > 0) launch_tables(gi);
+    for (size_t li = group_launch[gi]; li < group_launch[gi + 1]; ++li) {
+      const BlsLaunch& l = plan.launch[li];
+      const unsigned gx = (unsigned)(l.cta_end - l.cta_begin);
+      if (l.ghist)
+        bls_search_kernel<true><<<gx, l.W * 32, l.smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per,
+                                                              d_cta + l.cta_begin, out_stride, d_durbins, D,
+                                                              bin_duration, oversample, objective, l.stride, g_hist,
+                                                              fast, o0, o1, o2, o3, o4, o5, o6, ob);
       else
-        bls_search_kernel<false><<<grid, W * 32, smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per, p0, p1, P,
-                                                             d_durbins, D, bin_duration, oversample, objective, stride,
-                                                             nullptr, fast, bb, o0, o1, o2, o3, o4, o5, o6, ob);
+        bls_search_kernel<false><<<gx, l.W * 32, l.smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per,
+                                                               d_cta + l.cta_begin, out_stride, d_durbins, D,
+                                                               bin_duration, oversample, objective, l.stride, nullptr,
+                                                               fast, o0, o1, o2, o3, o4, o5, o6, ob);
     }
     LKB_LAUNCH_CHECK();
-    p0 = p1;
   }
   prof_end(st);
 

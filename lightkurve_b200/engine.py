@@ -297,8 +297,10 @@ BLS_FIELDS = ("power", "depth", "depth_err", "duration", "transit_time", "depth_
 
 def bls_power(times, fluxes, flux_errs, period, duration, oversample=10, objective="likelihood",
               return_bins=False):
-    """K3.  Lists of per-LC arrays (flux_errs: list or None => unit weights), one shared
-    period grid [P] and duration grid [D].  Returns dict of [B, P] float64 arrays."""
+    """K3.  Lists of per-LC arrays (flux_errs: list or None => unit weights) and one duration grid [D].
+    `period`: one grid [P] shared by all light curves - returns a dict of [B, P] float64 arrays - or a list of
+    B one-dimensional per-light-curve grids (one GPU call; each light curve's result is bitwise what a call on its own grid
+    gives) - then every field, "bins" and "period" included, is a list of per-light-curve arrays."""
     lib = L.load()
     B = len(times)
     t, offsets = _csr(times)
@@ -310,18 +312,32 @@ def bls_power(times, fluxes, flux_errs, period, duration, oversample=10, objecti
         dy, doff = _csr(flux_errs)
         if not np.array_equal(offsets, doff):
             raise ValueError("time and flux_err lengths differ")
-    period = np.ascontiguousarray(np.atleast_1d(period), dtype=np.float64)
     duration = np.ascontiguousarray(np.atleast_1d(duration), dtype=np.float64)
-    P, D = len(period), len(duration)
-    outs = [np.empty((B, P), dtype=np.float64) for _ in range(7)]
-    bins = np.empty((B, P, 2), dtype=np.int32) if return_bins else None
-    L.check(lib.lkb_bls_power(L.ptr(t), L.ptr(y), L.ptr(dy), L.ptr(offsets), B, L.ptr(period), P, L.ptr(duration), D,
-                              int(oversample), L.BLS_SNR if objective == "snr" else L.BLS_LIKELIHOOD,
-                              *[L.ptr(o) for o in outs], L.ptr(bins), L.MEM_HOST, None))
+    D = len(duration)
+    # a list of arrays is one grid per light curve; a list of numbers is one shared grid, as it always was
+    per_lc = isinstance(period, (list, tuple)) and len(period) > 0 and all(np.ndim(p) == 1 for p in period)
+    if per_lc:
+        if len(period) != B:
+            raise ValueError("%d period grids for %d light curves" % (len(period), B))
+        period, pofs = _csr([np.atleast_1d(p) for p in period])
+        P = int(pofs[-1])
+        shape = (P,)
+    else:
+        period = np.ascontiguousarray(np.atleast_1d(period), dtype=np.float64)
+        pofs = None
+        P = len(period)
+        shape = (B, P)
+    outs = [np.empty(shape, dtype=np.float64) for _ in range(7)]
+    bins = np.empty(shape + (2,), dtype=np.int32) if return_bins else None
+    L.check(lib.lkb_bls_power_ex(L.ptr(t), L.ptr(y), L.ptr(dy), L.ptr(offsets), B, L.ptr(period), L.ptr(pofs), P,
+                                 L.ptr(duration), D, int(oversample), L.BLS_SNR if objective == "snr" else L.BLS_LIKELIHOOD,
+                                 *[L.ptr(o) for o in outs], L.ptr(bins), L.MEM_HOST, None))
     res = dict(zip(BLS_FIELDS, outs))
     res["period"] = period
     if return_bins:
         res["bins"] = bins
+    if per_lc:
+        res = {k: [v[pofs[b]:pofs[b + 1]] for b in range(B)] for k, v in res.items()}
     return res
 
 

@@ -558,7 +558,7 @@ class BoxLeastSquaresPeriodogram(Periodogram):
     def _finish(prep, res, b=0):
         lc = prep["lc"]
         tu = u._as_unit(prep["time_unit"])
-        period = Quantity(res["period"], tu)
+        period = Quantity(res["period"][b] if isinstance(res["period"], list) else res["period"], tu)
         return BoxLeastSquaresPeriodogram(
             frequency=1.0 / period,
             power=Quantity(res["power"][b], u.dimensionless_unscaled),
