@@ -192,6 +192,14 @@ int lkb_flatten(const double* time, const double* flux, const double* flux_err,
                 const uint8_t* exclude_mask, const int64_t* offsets, int B,
                 int window_length, int polyorder, double break_tolerance, int niters, double sigma,
                 double* flat, double* flat_err, double* trend, int mem, void* stream);
+/* kernel path the most recent lkb_flatten call ran; -1 before the first call.  Which path runs follows from the
+ * window, the polyorder and the longest light curve (lightkurve_b200/csrc/flatten_plan.h). */
+#define LKB_FLATTEN_PATH_V2_MOMENTS 0   /* streaming kernel, interior from sliding moments */
+#define LKB_FLATTEN_PATH_V2_DIRECT  1   /* streaming kernel, interior from direct taps (short windows) */
+#define LKB_FLATTEN_PATH_V1         2   /* FIR kernel: polyorder > 5, window too long for a v2 tile, a light curve
+                                         * longer than 131072 cadences, or LKB_FLATTEN_V1 set */
+#define LKB_FLATTEN_PATH_V1_RERUN   3   /* FIR kernel after the streaming kernel found > 1022 gap cuts */
+int lkb_flatten_last_path(void);
 
 /* Host-only helper (no GPU needed): the Savitzky-Golay tables lkb_flatten uploads -
  * coeffs[w] = scipy.signal.savgol_coeffs(w, p) (symmetric FIR) and edge[w*(w/2)] with

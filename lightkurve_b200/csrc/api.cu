@@ -389,6 +389,8 @@ int lkb_flatten(const double* time, const double* flux, const double* flux_err, 
                  sigma, flat, flat_err, trend, mem, (cudaStream_t)stream);
 }
 
+int lkb_flatten_last_path(void) { return g_last_flatten_path; }
+
 int lkb_regress(const double* X, int x_batched, const double* y, const double* flux_err, const uint8_t* cadence_mask,
                 const double* prior_mu, const double* prior_sigma, int B, int64_t N, int K, double clip_sigma,
                 int niters, double* coeff, double* model, uint8_t* outlier_mask, int32_t* status_out,

@@ -13,6 +13,7 @@ namespace lkb {
 void set_error(const char* fmt, ...);
 extern int64_t g_launches;
 extern int g_last_ls_algo;
+extern int g_last_flatten_path;
 // ls_nufft.cu: light curves of the current / last shared-grid NUFFT call that took the double-precision pass
 void ls_nufft_begin_call(cudaStream_t st);
 int ls_nufft_last_escalated();

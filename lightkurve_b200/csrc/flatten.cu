@@ -15,6 +15,8 @@
 
 namespace lkb {
 
+int g_last_flatten_path = -1;      // kernel path of the last lkb_flatten call (LKB_FLATTEN_PATH_*; -1: none yet)
+
 constexpr int FL_THREADS = 512;
 constexpr int FL_R = 4;                          // outputs per thread per tile
 constexpr int FL_TI = FL_THREADS * FL_R;         // outputs per tile
@@ -325,16 +327,22 @@ static bool solve_dense(std::vector<double>& A, std::vector<double>& Bm, int n, 
 }
 
 // Projection matrix H = V (V^T V)^-1 V^T of the degree-p least-squares fit on w equispaced
-// abscissae (Legendre-like scaling u = (k - c)/c keeps V^T V well conditioned).
-// coeffs[j] = H[center][j] (symmetric FIR); edge[j*half + i] = H[i][j], i < half.
+// abscissae u = (k - c)/c in [-1, 1].  The columns of V are the Legendre polynomials P_r(u), nearly
+// orthogonal on these points, so V^T V stays well conditioned up to polyorder 12 (monomials u^r lose
+// ~1e-8 of the taps there).  coeffs[j] = H[center][j] (symmetric FIR); edge[j*half + i] = H[i][j], i < half.
 static bool savgol_tables(int w, int p, std::vector<double>& coeffs, std::vector<double>& edge) {
   const int q = p + 1, half = w / 2;
   const double c = 0.5 * (w - 1), sc = c > 0 ? c : 1.0;
   std::vector<double> V((size_t)w * q);
   for (int k = 0; k < w; ++k) {
     const double u = (k - c) / sc;
-    double pw = 1.0;
-    for (int r = 0; r < q; ++r) { V[(size_t)k * q + r] = pw; pw *= u; }
+    double p0 = 1.0, p1 = u;
+    for (int r = 0; r < q; ++r) {
+      V[(size_t)k * q + r] = p0;
+      const double p2 = ((2 * r + 3) * u * p1 - (r + 1) * p0) / (r + 2);     // (r+2) P_{r+2} = (2r+3) u P_{r+1} - (r+1) P_r
+      p0 = p1;
+      p1 = p2;
+    }
   }
   std::vector<double> G((size_t)q * q, 0.0), Vt((size_t)q * w);
   for (int r = 0; r < q; ++r)
@@ -398,6 +406,35 @@ int savgol_tables_host(int w, int p, double* coeffs, double* edge) {
   return LKB_OK;
 }
 
+struct F2Args {
+  const double *t, *f, *fe;
+  const uint8_t* ex;
+  const int64_t* off;
+  double* tro;
+  int window_length;
+  double break_tolerance;
+  int niters;
+  double sigma;
+  F2Coef cf;
+  int tile_out;
+  double *flat, *flat_err, *trend;
+  int* status;
+};
+
+template <int NM, bool DIRECT>
+static int launch_flatten2(const F2Args& a, int B, size_t smem, cudaStream_t st) {
+  static size_t attr = 0;
+  auto* kernel = flatten2_kernel<NM, DIRECT>;
+  if (smem > attr) {
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = smem;
+  }
+  kernel<<<B, F2_THREADS, smem, st>>>(a.t, a.f, a.fe, a.ex, a.off, a.tro, a.window_length,
+                                      a.break_tolerance, a.niters, a.sigma, a.cf, a.tile_out, a.flat, a.flat_err,
+                                      a.trend, a.status);
+  return LKB_OK;
+}
+
 int flatten(const double* time, const double* flux, const double* flux_err, const uint8_t* exclude_mask,
             const int64_t* h_offsets, int B, int window_length, int polyorder, double break_tolerance, int niters,
             double sigma, double* flat, double* flat_err, double* trend, int mem, cudaStream_t st) {
@@ -441,41 +478,29 @@ int flatten(const double* time, const double* flux, const double* flux_err, cons
   LKB_TRY(stage_out_alloc<double>(mem, WS_OUT1, flat_err, total, &o_fe));
   LKB_TRY(stage_out_alloc<double>(mem, WS_OUT2, trend, total, &o_tr));
 
-  // ---- v2 kernel (flatten_v2.cuh: bitmask bookkeeping, sliding-moment Savitzky-Golay) whenever the shapes allow ----
+  // ---- v2 kernel (flatten_v2.cuh: bitmask bookkeeping, sliding-moment or direct-tap Savitzky-Golay) whenever the
+  // plan allows (flatten_plan.h) ----
+  int64_t nmax = 0;
+  for (int b = 0; b < B; ++b) nmax = std::max(nmax, h_offsets[b + 1] - h_offsets[b]);
+  const FlattenPlan plan = flatten_plan(window_length, polyorder, nmax);
+  g_last_flatten_path = LKB_FLATTEN_PATH_V1;
   {
-    int64_t nmax = 0;
-    for (int b = 0; b < B; ++b) nmax = std::max(nmax, h_offsets[b + 1] - h_offsets[b]);
-    const int NM = polyorder <= 1 ? 1 : polyorder <= 3 ? 3 : 5;
-    int tile_out = std::min(2048, std::min(65536 / (8 * NM) - 2 * half - 1, 4094 - 2 * half));
-    // fourth-order power sums lose (tile half-length / half-window)^4 in the difference of prefix sums: short tiles
-    if (NM == 5) tile_out = std::min(tile_out, std::max(128, 10 * half));
+    const int NM = plan.nm, tile_out = plan.tile_out;
     F2Coef cf;
-    if (!getenv("LKB_FLATTEN_V1") && polyorder <= 5 && nmax <= F2_MAXN && tile_out >= 128 &&
-        savgol_ginv(window_length, polyorder, cf)) {
+    if (!getenv("LKB_FLATTEN_V1") && plan.route == FLATTEN_V2 && savgol_ginv(window_length, polyorder, cf)) {
       double* tro = nullptr;
       int* d_status = nullptr;
       LKB_TRY(ws_get_t<double>(WS_H, total, &tro));
       LKB_TRY(ws_get_t<int>(WS_N, B, &d_status));
       const size_t smem2 = ((sizeof(F2Smem) + 15) & ~(size_t)15) +
                            sizeof(double) * std::max((size_t)NM * (tile_out + 2 * half + 1), (size_t)(FS_CAP + FS_SAMPLE));
-      static size_t attr2[3] = {0, 0, 0};
-      const int slot = NM == 1 ? 0 : NM == 3 ? 1 : 2;
-      if (smem2 > attr2[slot]) {
-        if (NM == 1) LKB_CUDA_CHECK(cudaFuncSetAttribute(flatten2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        else if (NM == 3) LKB_CUDA_CHECK(cudaFuncSetAttribute(flatten2_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        else LKB_CUDA_CHECK(cudaFuncSetAttribute(flatten2_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        attr2[slot] = smem2;
-      }
       prof_begin(st);
-      if (NM == 1)
-        flatten2_kernel<1><<<B, F2_THREADS, smem2, st>>>(d_t, d_f, d_fe, d_ex, d_off, tro, window_length, break_tolerance,
-                                                      niters, sigma, cf, tile_out, o_flat, o_fe, o_tr, d_status);
-      else if (NM == 3)
-        flatten2_kernel<3><<<B, F2_THREADS, smem2, st>>>(d_t, d_f, d_fe, d_ex, d_off, tro, window_length, break_tolerance,
-                                                      niters, sigma, cf, tile_out, o_flat, o_fe, o_tr, d_status);
-      else
-        flatten2_kernel<5><<<B, F2_THREADS, smem2, st>>>(d_t, d_f, d_fe, d_ex, d_off, tro, window_length, break_tolerance,
-                                                      niters, sigma, cf, tile_out, o_flat, o_fe, o_tr, d_status);
+      const F2Args a{d_t, d_f, d_fe, d_ex, d_off, tro, window_length, break_tolerance, niters, sigma, cf, tile_out,
+                     o_flat, o_fe, o_tr, d_status};
+      const int rc = NM == 1 ? launch_flatten2<1, false>(a, B, smem2, st)
+                     : NM == 3 ? (plan.direct ? launch_flatten2<3, true>(a, B, smem2, st) : launch_flatten2<3, false>(a, B, smem2, st))
+                     : (plan.direct ? launch_flatten2<5, true>(a, B, smem2, st) : launch_flatten2<5, false>(a, B, smem2, st));
+      LKB_TRY(rc);
       prof_end(st);
       LKB_LAUNCH_CHECK();
       std::vector<int> h_status(B, 0);
@@ -484,6 +509,7 @@ int flatten(const double* time, const double* flux, const double* flux_err, cons
       bool overflow = false;
       for (int b = 0; b < B; ++b) overflow = overflow || h_status[b] == 2;
       if (!overflow) {
+        g_last_flatten_path = plan.direct ? LKB_FLATTEN_PATH_V2_DIRECT : LKB_FLATTEN_PATH_V2_MOMENTS;
         LKB_TRY(stage_out_copy<double>(mem, flat, o_flat, total, st));
         LKB_TRY(stage_out_copy<double>(mem, flat_err, o_fe, total, st));
         LKB_TRY(stage_out_copy<double>(mem, trend, o_tr, total, st));
@@ -491,6 +517,7 @@ int flatten(const double* time, const double* flux, const double* flux_err, cons
         return LKB_OK;
       }
       // a light curve with more gap segments than the v2 kernel's shared-memory list: the whole call re-runs below
+      g_last_flatten_path = LKB_FLATTEN_PATH_V1_RERUN;
     }
   }
 

@@ -10,7 +10,9 @@
 //   * Savitzky-Golay by SLIDING MOMENTS (SURVEY.md H7): the centre tap of a degree-p least-squares fit over a
 //     symmetric window is an even polynomial in the offset j,  c_j = A0 + A2 j^2 (+ A4 j^4),  so
 //     y_k = sum_s A_s sum_j j^s x_{k+j}  and the windowed power sums are differences of prefix sums of q^s x_q over a
-//     tile (q measured from the tile centre, fp64: ~1e-12 relative) - O(1) per output instead of O(window);
+//     tile (q measured from the tile centre) - O(1) per output instead of O(window).  Their rounding grows with the
+//     tile and is amplified by the re-centring as the window shrinks, so short windows (flatten_plan.h: where the
+//     predicted error exceeds F2_MOMENT_TOL) take the direct dot product of the centre taps with the staged inputs;
 //   * the segment edges are the degree-p polynomial fitted to the first / last `window` samples (scipy
 //     _fit_edges_polyfit) evaluated from its p + 1 moments (one block reduction per edge) instead of a
 //     [window x window/2] table product;
@@ -18,16 +20,16 @@
 //     intermediate ones, lightcurve.py:1053-1058), fused with flux / trend and flux_err / trend.
 // Global memory per iteration: t once (gap statistics), f once + trend-at-kept written (filter), f + trend read
 // (residual clip); order statistics by the radix select of select.cuh on functors that read through the bitmask.
-// Supported: polyorder <= 5, window <= 2047, n <= 131072 per light curve, <= 1023 gap segments; anything else (and a
-// light curve that overflows the segment list, status 2) runs flatten.cu's first kernel.
+// Supported: polyorder <= 5, a tile of >= 128 outputs, n <= F2_MAXN per light curve (flatten_plan.h), <= 1023 gap
+// segments; anything else (and a light curve that overflows the segment list, status 2) runs flatten.cu's first kernel.
 #pragma once
 #include "common.cuh"
 #include "select.cuh"
+#include "flatten_plan.h"
 
 namespace lkb {
 
 constexpr int F2_THREADS = 512;
-constexpr int F2_MAXN = 131072;
 constexpr int F2_MAXWORDS = F2_MAXN / 32;
 constexpr int F2_MAXSEG = 1024;
 constexpr int F2_MAXQ = 6;                      // polyorder + 1
@@ -159,14 +161,16 @@ __device__ inline void f2_block_sums(F2Smem& sm, const double* v, int nq) {
   __syncthreads();
 }
 
-// NM = number of prefix-sum arrays (power sums q^0 .. q^(NM-1)): 1 for polyorder <= 1, 3 for <= 3, 5 for <= 5
-template <int NM>
+// NM = number of prefix-sum arrays (power sums q^0 .. q^(NM-1)): 1 for polyorder <= 1, 3 for <= 3, 5 for <= 5;
+// DIRECT: the interior from the centre taps instead of the moments (flatten_plan.h), NM = 3 and 5 only
+template <int NM, bool DIRECT = false>
 __global__ void __launch_bounds__(F2_THREADS, 2)
 flatten2_kernel(const double* __restrict__ time, const double* __restrict__ flux, const double* __restrict__ flux_err,
                 const uint8_t* __restrict__ exclude, const int64_t* __restrict__ offsets, double* __restrict__ tro_ws,
                 int window_length, double break_tolerance, int niters, double sigma, F2Coef cf, int tile_out,
                 double* __restrict__ flat, double* __restrict__ flat_err, double* __restrict__ trend,
                 int* __restrict__ status) {
+  static_assert(!DIRECT || NM >= 3, "direct taps replace the moments of polyorder >= 2");
   LKB_DYN_SMEM(unsigned char, f2_dyn);
   F2Smem& sm = *reinterpret_cast<F2Smem*>(f2_dyn);
   double* P = reinterpret_cast<double*>(f2_dyn + ((sizeof(F2Smem) + 15) & ~(size_t)15));     // NM arrays of plen doubles
@@ -346,6 +350,14 @@ flatten2_kernel(const double* __restrict__ time, const double* __restrict__ flux
       if (r == r) { rs1 += r; rs2 = fma(r, r, rs2); rsc++; }
     };
     // ---- Savitzky-Golay interior by tiles of `tile_out` kept positions ----
+    // direct taps: c_j = A0 + A1 j^2 + A2 j^4 for j = 0 .. half in the second array (idle without moments; written
+    // every iteration because the select's candidate buffer aliases it; the first f2_select4 publishes them)
+    double* taps = P + plen;
+    if (DIRECT)
+      for (int j = t; j <= half; j += F2_THREADS) {
+        const double j2 = (double)j * (double)j;
+        taps[j] = fma(fma(cf.A[2], j2, cf.A[1]), j2, cf.A[0]);
+      }
     for (int k0 = 0; k0 < m; k0 += tile_out) {
       const int kin0 = max(0, k0 - half), kin1 = min(m, k0 + tile_out + half);      // inputs [kin0, kin1)
       const int kout1 = min(m, k0 + tile_out);
@@ -372,7 +384,7 @@ flatten2_kernel(const double* __restrict__ time, const double* __restrict__ flux
       }
       __syncthreads();
       // prefix sums P[s][q + 1] = sum_{q' <= q} (q' - qc)^s x_q'   (each thread owns PER consecutive q)
-      {
+      if (!DIRECT) {
         const int PER = (nin + F2_THREADS - 1) / F2_THREADS;
         const int q0 = t * PER, q1 = min(nin, q0 + PER);
         double run[NM];
@@ -432,6 +444,14 @@ flatten2_kernel(const double* __restrict__ time, const double* __restrict__ flux
         const int len = h - l;
         if ((w > len) || ((double)len < break_tolerance)) continue;          // median fallback (below)
         if (k - l < half || h - k <= half) continue;                           // edge (below)
+        if (DIRECT) {
+          const double* xk = P + (k - kin0 + 1);
+          double y = taps[0] * xk[0];
+          for (int j = 1; j <= half; ++j) y = fma(taps[j], xk[-j] + xk[j], y);
+          tro[i] = y;
+          residual(i, y);
+          continue;
+        }
         const int a = k - half - kin0, e = k + half - kin0 + 1;                // window [a, e) in tile coordinates
         const double kc = (double)(k - kin0) - qc;
         const double S0 = P[e] - P[a];

@@ -47,6 +47,13 @@ def ls_last_algo():
         int(L.load().lkb_ls_last_algo()), "none")
 
 
+def flatten_last_path():
+    """Kernel path the most recent flatten call ran: "v2-moments" or "v2-direct" (streaming kernel, interior from
+    sliding moments or direct taps), "v1" (FIR kernel) or "v1-rerun" (FIR kernel after more than 1022 gap cuts)."""
+    return {L.FLATTEN_PATH_V2_MOMENTS: "v2-moments", L.FLATTEN_PATH_V2_DIRECT: "v2-direct", L.FLATTEN_PATH_V1: "v1",
+            L.FLATTEN_PATH_V1_RERUN: "v1-rerun"}.get(int(L.load().lkb_flatten_last_path()), "none")
+
+
 def ls_last_escalated():
     """Light curves of the most recent shared-grid NUFFT call that took the double-precision pass (lkb200.h)."""
     return int(L.load().lkb_ls_last_escalated())

@@ -2,7 +2,11 @@
 
 flatten   : /root/reference/src/lightkurve/lightcurve.py:996-1070 restated on plain
             ndarrays; calls the REAL scipy.signal.savgol_filter (:1040) and
-            scipy.interpolate.interp1d (:1053) the reference calls.
+            scipy.interpolate.interp1d (:1053) the reference calls.  savgol=savgol_lsq
+            swaps in the same filter from a well-conditioned least-squares basis:
+            scipy builds its taps from the unscaled Vandermonde matrix of the window
+            offsets, which loses accuracy at polyorder >= 4 and long windows (taps off
+            by 1e-8 relative at window 201, 1e-6 at 1001, for polyorder 5).
 sigma_clip: astropy.stats.sigma_clip defaults (maxiters=5, median, std) as used at
             correctors/regressioncorrector.py:269 -- restated (astropy absent).
 regress   : correctors/regressioncorrector.py:127-189 (_fit_coefficients, dense
@@ -11,16 +15,45 @@ normalize : lightcurve.py:1253-1254.
 Pinned by the reference's known-answer tests (tests/test_lightcurve.py:1284-1360,
 tests/correctors/test_regressioncorrector.py:13-83) ported under tests/.
 """
+import functools
 import warnings
 
 import numpy as np
+from numpy.polynomial import legendre
 from scipy.interpolate import interp1d
 from scipy.signal import savgol_filter
 
 
+@functools.lru_cache(maxsize=64)
+def _savgol_basis(window_length, polyorder):
+    """Orthonormal basis [window_length, polyorder + 1] of the polynomials of degree <= polyorder on the window:
+    QR of the Legendre Vandermonde matrix on u = (k - half) / half, whose columns are nearly orthogonal."""
+    half = window_length // 2
+    u = (np.arange(window_length) - half) / max(half, 1)
+    q, _ = np.linalg.qr(legendre.legvander(u, polyorder))
+    q.setflags(write=False)
+    return q
+
+
+def savgol_lsq(x, window_length, polyorder):
+    """scipy.signal.savgol_filter(x, window_length, polyorder) (mode="interp", len(x) >= window_length): the
+    least-squares polynomial of the window around each interior point evaluated at its centre, and the fits of the
+    first and last windows evaluated at the edge points; the projections come from _savgol_basis."""
+    x = np.asarray(x, dtype=np.float64)
+    n, w, half = len(x), window_length, window_length // 2
+    q = _savgol_basis(w, polyorder)
+    taps = q @ q[half]
+    y = np.empty(n)
+    y[half:n - half] = np.convolve(x, taps[::-1], mode="valid")
+    y[:half] = q[:half] @ (q.T @ x[:w])
+    y[n - half:] = q[w - half:] @ (q.T @ x[n - w:])
+    return y
+
+
 def flatten(time, flux, flux_err=None, window_length=101, polyorder=2, break_tolerance=5,
-            niters=3, sigma=3, mask=None):
-    """Returns (flat_flux, flat_flux_err, trend).  `mask` True = exclude (lightcurve.py:980-1000)."""
+            niters=3, sigma=3, mask=None, savgol=savgol_filter):
+    """Returns (flat_flux, flat_flux_err, trend).  `mask` True = exclude (lightcurve.py:980-1000).  `savgol`: the
+    Savitzky-Golay filter, called as savgol(x, window_length, polyorder)."""
     time = np.asarray(time, dtype=np.float64)
     flux = np.asarray(flux)
     if not np.issubdtype(flux.dtype, np.floating):
@@ -58,8 +91,7 @@ def flatten(time, flux, flux_err=None, window_length=101, polyorder=2, break_tol
             if np.any([window_length > (h - l), (h - l) < break_tolerance]):
                 trend_signal[l:h] = np.nanmedian(fm[l:h])
             else:
-                trend_signal[l:h] = savgol_filter(x=fm[l:h], window_length=window_length,
-                                                  polyorder=polyorder)
+                trend_signal[l:h] = savgol(fm[l:h], window_length, polyorder)
         with warnings.catch_warnings():
             warnings.simplefilter("ignore", RuntimeWarning)
             mask1 = np.nan_to_num(np.abs(fm - trend_signal)) < (np.nanstd(fm - trend_signal) * sigma + 1e-14)

@@ -5,11 +5,14 @@ import ctypes
 import os
 import shutil
 import subprocess
+from fractions import Fraction
 
 import numpy as np
 import pytest
+import scipy.signal
 
 from oracle import detrend as odet
+from test_gpu_flatten_paths import F2_MAXN, plan
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CUDA_INC = "/usr/local/cuda/include"
@@ -27,6 +30,7 @@ def emu(tmp_path_factory):
 
 
 def _bind(lib):
+    lib.emu_flatten_plan.argtypes = [c_int, c_int, ctypes.c_int64, c_vp, c_vp]
     lib.emu_flatten2.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_dbl, c_int, c_dbl, c_vp, c_vp, c_int,
                                  c_vp, c_vp, c_vp, c_vp]
     return lib
@@ -58,17 +62,11 @@ def _run(emu, times, fluxes, errs, masks, w, p, bt, niters, sigma, tile_out=None
     fe = np.ascontiguousarray(np.concatenate(errs))
     ex = None if masks is None else np.ascontiguousarray(np.concatenate(masks).astype(np.uint8))
     A, Ginv = _coef(w, p)
-    NM = 1 if p <= 1 else 3 if p <= 3 else 5
-    half = w // 2
-    if tile_out is None:
-        tile_out = min(2048, 65536 // (8 * NM) - 2 * half - 1, 4094 - 2 * half)
-        if NM == 5:
-            tile_out = min(tile_out, max(128, 10 * half))         # (flatten.cu: precision of the fourth-order sums)
     flat, flat_err, trend = (np.full(len(t), -7.0) for _ in range(3))
     status = np.full(B, -1, np.int32)
     emu.emu_flatten2(t.ctypes.data, f.ctypes.data, fe.ctypes.data, None if ex is None else ex.ctypes.data, off.ctypes.data, B,
                      w, p, np.nan if bt is None else float(bt), niters, float(sigma), A.ctypes.data, Ginv.ctypes.data,
-                     tile_out, flat.ctypes.data, flat_err.ctypes.data, trend.ctypes.data, status.ctypes.data)
+                     tile_out or 0, flat.ctypes.data, flat_err.ctypes.data, trend.ctypes.data, status.ctypes.data)
     sp = lambda a: [a[off[b]:off[b + 1]] for b in range(B)]
     return sp(flat), sp(flat_err), sp(trend), status
 
@@ -174,3 +172,81 @@ def test_flatten_v2_mask_and_failure_on_the_emulator(emu):
     np.testing.assert_allclose(trend[0], rt, rtol=1e-9)
     np.testing.assert_allclose(flat[0], rf, rtol=1e-9)
     assert np.isnan(trend[1]).all() and np.isnan(flat[1]).all()
+
+
+def test_plan_restated_in_python_matches_flatten_plan_h(emu):
+    """tests/test_gpu_flatten_paths.py::plan (the GPU tests' expected paths) against flatten_plan.h itself."""
+    routes = {0: "v2", 1: "polyorder", 2: "tile", 3: "length"}
+    tile, direct = c_int(), c_int()
+    for w in list(range(1, 300, 2)) + list(range(301, 8192, 34)) + [1509, 1511, 2601, 2603, 3967, 3969, 8191]:
+        for p in range(min(w, 13)):
+            for nmax in (1000, F2_MAXN, F2_MAXN + 1):
+                r = emu.emu_flatten_plan(w, p, nmax, ctypes.byref(tile), ctypes.byref(direct))
+                assert (routes[r], tile.value, bool(direct.value)) == tuple(plan(w, p, nmax)[i] for i in (0, 2, 3)), (w, p, nmax)
+
+
+def _exact_rows(w, p, rows):
+    """Rows i of the least-squares projection onto degree-p polynomials over w equispaced points, exact (rational)."""
+    xs = [k - w // 2 for k in range(w)]
+    q = p + 1
+    M = [[Fraction(sum(x ** (r + s) for x in xs)) for s in range(q)] + [Fraction(int(r == s)) for s in range(q)]
+         for r in range(q)]
+    for c in range(q):                                                # Gauss-Jordan: M = [G | I] -> [I | G^-1]
+        piv = next(r for r in range(c, q) if M[r][c] != 0)
+        M[c], M[piv] = M[piv], M[c]
+        M[c] = [v / M[c][c] for v in M[c]]
+        for r in range(q):
+            if r != c and M[r][c] != 0:
+                M[r] = [a - M[r][c] * b for a, b in zip(M[r], M[c])]
+    gi = [row[q:] for row in M]
+    out = []
+    for i in rows:
+        a = [sum(xs[i] ** r * gi[r][s] for r in range(q)) for s in range(q)]
+        out.append([float(sum(a[s] * x ** s for s in range(q))) for x in xs])
+    return np.array(out)
+
+
+@pytest.mark.parametrize("w,p", [(5, 2), (7, 4), (21, 5), (101, 2), (201, 5), (1001, 5), (51, 12), (401, 12), (13, 12)])
+def test_savgol_lsq_matches_exact_taps(w, p):
+    """oracle.detrend.savgol_lsq (the GPU tests' reference filter) against exact rational least squares: centre taps
+    and edge rows to 1e-13 of sum |tap| max |x|; and against scipy.signal.savgol_filter where scipy's own taps are
+    accurate (polyorder <= 3)."""
+    half = w // 2
+    rows = [half, 0, half - 1]
+    exact = _exact_rows(w, p, rows)
+    rng = np.random.default_rng(w + p)
+    x = rng.normal(size=3 * w)
+    y = odet.savgol_lsq(x, w, p)
+    tol = lambda taps: 1e-13 * np.abs(taps).sum() * np.abs(x).max()
+    np.testing.assert_allclose(y[half:len(x) - half], np.convolve(x, exact[0][::-1], mode="valid"), rtol=0,
+                               atol=tol(exact[0]))
+    np.testing.assert_allclose(y[0], exact[1] @ x[:w], rtol=0, atol=tol(exact[1]))
+    np.testing.assert_allclose(y[half - 1], exact[2] @ x[:w], rtol=0, atol=tol(exact[2]))
+    if p <= 3:
+        np.testing.assert_allclose(y, scipy.signal.savgol_filter(x, w, p), rtol=0, atol=1e-12 * np.abs(x).max())
+
+
+# (window, polyorder) of the short windows and of polyorder 4-5, the cases whose interior the sliding moments of
+# flatten_v2.cuh got wrong by up to 8e-8 before the direct taps (flatten_plan.h)
+SHORT_AND_QUARTIC = [(5, 3), (7, 2), (9, 2), (11, 2), (15, 2), (15, 3), (21, 2), (25, 3), (31, 2), (7, 4), (7, 5), (9, 4),
+                     (11, 5), (21, 4), (41, 5), (75, 4), (101, 4), (101, 5), (201, 5), (401, 5), (1001, 5), (3, 1),
+                     (1001, 1)]
+
+
+@pytest.mark.parametrize("w,p", SHORT_AND_QUARTIC, ids=["w%d-p%d" % c for c in SHORT_AND_QUARTIC])
+def test_flatten_v2_short_windows_and_quartic_on_the_emulator(emu, w, p):
+    """flatten.cu's plan (tile and interior method) on 3000 + 1200 cadences with gaps and outliers, flux ~1 or in
+    e-/s, against the reference flatten body with the well-conditioned filter (scipy's own taps are off by up to 1e-6
+    at polyorder 5 and long windows): trend, flat and flat_err to rtol 1e-9."""
+    rng = np.random.default_rng(7 * w + p)
+    lcs = [_lc(rng, n) for n in (3000, 1200)]
+    if (w + p) % 2:
+        lcs = [(t, 1e5 * f, 1e5 * fe) for t, f, fe in lcs]
+    times, fluxes, errs = (list(x) for x in zip(*lcs))
+    flat, flat_err, trend, status = _run(emu, times, fluxes, errs, None, w, p, 5, 3, 3)
+    assert (status == 0).all(), status
+    for b in range(len(times)):
+        rf, re_, rt = odet.flatten(times[b], fluxes[b], errs[b], window_length=w, polyorder=p, savgol=odet.savgol_lsq)
+        np.testing.assert_allclose(trend[b], rt, rtol=1e-9)
+        np.testing.assert_allclose(flat[b], rf, rtol=1e-9, equal_nan=True)
+        np.testing.assert_allclose(flat_err[b], re_, rtol=1e-9, equal_nan=True)

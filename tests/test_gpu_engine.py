@@ -474,8 +474,8 @@ def test_flatten_kernel_generations_agree(engine, monkeypatch):
     np.testing.assert_allclose(trend[0], rt, rtol=1e-9)
     np.testing.assert_allclose(flat[0], rf, rtol=1e-9)
     flat6, _, trend6 = engine.flatten([lcs[1][0]], [lcs[1][1]], [lcs[1][2]], None, window_length=51, polyorder=6)
-    np.testing.assert_allclose(trend6[0], odet.flatten(lcs[1][0], lcs[1][1], lcs[1][2], window_length=51, polyorder=6)[2],
-                               rtol=2e-7)      # (first kernel: degree-6 edge tables)
+    np.testing.assert_allclose(trend6[0], odet.flatten(lcs[1][0], lcs[1][1], lcs[1][2], window_length=51, polyorder=6,
+                                                       savgol=odet.savgol_lsq)[2], rtol=1e-9)
 
 
 def test_flatten_reference_known_answers(engine):
