@@ -76,6 +76,10 @@ int lkb_ls_last_algo(void);
 /* light curves of the most recent shared-grid NUFFT call that were transformed a second time in double precision
  * (precision escalation: flux excursion > LKB_NUFFT_ESCALATE [250] x the in-band peak amplitude; DESIGN.md section 2) */
 int lkb_ls_last_escalated(void);
+/* transform of the most recent NUFFT call (any entry): out[0] = 1 for the v2 transform (one real transform per light
+ * curve), 0 for the round-1 pair-packed one (only on request, LKB_NUFFT_FFT), -1 before the first NUFFT call;
+ * out[1] = p, out[2] = p2: the flux and window-term fine grids have 2^p and 2^p2 cells.  Returns LKB_OK. */
+int lkb_ls_last_nufft_plan(int* out3);
 /* Measurement hooks (bench.py roofline): when enabled, every compute call records CUDA events on
  * its stream around its DOMINANT kernel (LS contraction / BLS search / flatten / Gram accumulation).
  * lkb_profile_read synchronises, writes up to max_n durations [ms] in call order, resets the ring

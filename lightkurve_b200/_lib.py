@@ -35,6 +35,7 @@ SIGNATURES = {
     "lkb_launch_count": (c_i64, []),
     "lkb_ls_last_algo": (c_int, []),
     "lkb_ls_last_escalated": (c_int, []),
+    "lkb_ls_last_nufft_plan": (c_int, [c_vp]),
     "lkb_profile_enable": (c_int, [c_int]),
     "lkb_profile_read": (c_int, [c_vp, c_int]),
     "lkb_ws_read": (c_int, [c_int, c_i64, c_i64, c_vp]),

@@ -303,6 +303,11 @@ int lkb_profile_read(double* ms_out, int max_n) {
 int64_t lkb_launch_count(void) { return g_launches; }
 int lkb_ls_last_algo(void) { return g_last_ls_algo; }
 int lkb_ls_last_escalated(void) { return g_last_ls_algo == LKB_LS_ALGO_NUFFT ? ls_nufft_last_escalated() : 0; }
+int lkb_ls_last_nufft_plan(int* out3) {
+  if (!out3) return LKB_E_ARG;
+  ls_nufft_last_plan(out3);
+  return LKB_OK;
+}
 
 // Diagnostic: copy `bytes` bytes at `offset` of workspace slot `slot` to the host buffer `out` (after a device
 // synchronise).  Lets a test or tools/nufft_gpu_check.py look at the intermediate buffers of the last call.

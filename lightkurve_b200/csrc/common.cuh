@@ -17,6 +17,7 @@ extern int g_last_flatten_path;
 // ls_nufft.cu: light curves of the current / last shared-grid NUFFT call that took the double-precision pass
 void ls_nufft_begin_call(cudaStream_t st);
 int ls_nufft_last_escalated();
+void ls_nufft_last_plan(int* out);
 extern int64_t g_epoch;
 
 #define LKB_CUDA_CHECK(expr)                                                        \

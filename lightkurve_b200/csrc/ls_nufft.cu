@@ -572,7 +572,8 @@ int fft_passes(float2* a, float2* b, int p, int npairs, cudaStream_t st, float2*
 // the column kernel's load phase (the fine grids are written once, already half transformed)
 // "v2" (nufft_v2.cuh; default where the fine grid allows it, 2^14 .. 2^23 cells) = one real transform per light
 // curve, pruned + tiled, table twiddles, finish fused into the row kernel; "global" = the pair-packed round-1 form
-// with one global sweep per radix pass (also what tiny and huge grids use).
+// with one global sweep per radix pass (also the window terms' transform of the shared-grid plan; the single-term flux
+// transforms take it only on request, single_term_log2 below).
 int fft_mode(int p = 0) {
   const char* e = getenv("LKB_NUFFT_FFT");
   if (e && strcmp(e, "smem") == 0) return 1;
@@ -625,6 +626,20 @@ double upsampling_min() {
   return s < 1.25 ? 1.25 : (s > 2.0 ? 2.0 : s);
 }
 int fine_log2(int64_t kmax_plus_1) { return nufft::fine_grid_log2(kmax_plus_1, upsampling_min()); }
+// Flux grid of the single-term transforms (shared and ragged): at least 2^V2R_P_MIN cells, so that every grid takes the
+// v2 transform - one real transform per light curve, whose result does not depend on its neighbours in the batch.
+// Below 2^14 cells the round-1 form packed two light curves into one complex transform, and the fp32 rounding of a
+// loud light curve's peak leaked into its quiet partner (DESIGN.md section 2).  Only the grid grows: sigma =
+// min(2, grid_sigma) stays 2, so the kernel width and shape stay those of the smallest grid.  LKB_NUFFT_FFT =
+// global / smem / fused asks for the round-1 transforms and keeps their grid size.
+bool round1_requested() {
+  const char* e = getenv("LKB_NUFFT_FFT");
+  return e && (strcmp(e, "global") == 0 || strcmp(e, "smem") == 0 || strcmp(e, "fused") == 0);
+}
+int single_term_log2(int64_t kmax_plus_1) {
+  const int p = fine_log2(kmax_plus_1);
+  return round1_requested() ? p : std::max(p, V2R_P_MIN);
+}
 int kernel_width(double sigma) {
   int w = nufft::es_width(sigma);
   if (const char* e = getenv("LKB_NUFFT_W")) w = atoi(e);
@@ -672,6 +687,16 @@ struct NufftPlan {
   int64_t Npad;
 };
 static NufftPlan g_plan;
+// transform and grid sizes of the most recent NUFFT call: {1 = v2 / 0 = round-1 pair-packed, p, p2} (diagnostic)
+static int g_last_plan[3] = {-1, 0, 0};
+static void record_plan(bool v2, int p, int p2) {
+  g_last_plan[0] = v2 ? 1 : 0;
+  g_last_plan[1] = p;
+  g_last_plan[2] = p2;
+}
+void ls_nufft_last_plan(int* out) {
+  for (int i = 0; i < 3; ++i) out[i] = g_last_plan[i];
+}
 
 // light curves that took the double-precision pass since the last ls_nufft_begin_call (diagnostic; synchronises)
 void ls_nufft_begin_call(cudaStream_t st) {
@@ -691,7 +716,8 @@ int ls_nufft_last_escalated() {
 int ls_nufft_prepare(const double* d_t, int64_t N, int64_t F, double grid_f0, double grid_df, float4* d_rot,
                      float2* d_rot2, int64_t F_low, cudaStream_t st, const double* d_freq, int64_t Npad) {
   const int64_t k0 = (int64_t)rint(grid_f0 / grid_df);
-  const int p = fine_log2(k0 + F), p2 = fine_log2(2 * (k0 + F));
+  // p2: the window terms' grid (one transform of unit strengths, y-independent)
+  const int p = single_term_log2(k0 + F), p2 = fine_log2(2 * (k0 + F));
   const double sigma = fmin(2.0, nufft::grid_sigma(p, k0 + F));   // (the validated rule: beta = 2.30 w from sigma = 2 on)
   const int w = kernel_width(sigma);
   const float beta = (float)nufft::es_beta(w, sigma);
@@ -798,6 +824,7 @@ int ls_nufft_prepare(const double* d_t, int64_t N, int64_t F, double grid_f0, do
   g_plan.cad = cad;
   g_plan.fge = fge;
   g_plan.dec = dec;
+  record_plan(v2, p, p2);
   return LKB_OK;
 }
 
@@ -1459,8 +1486,16 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
   (void)h_off;
   int64_t k0 = 0;
   LKB_TRY(ragged_grid_check(B, h_span, f0, df, &k0));
-  const int p = fine_log2(k0 + F), p2 = fine_log2(2 * (k0 + F));
+  // flux grid 2^p, window grid 2^p2 = 2^(p + 1).  Both must be in the v2 range: above it (2^20 < k0 + F) the call is
+  // refused and `auto` runs the direct kernel, rather than pair-packing the window grid (LKB_NUFFT_FFT = global /
+  // smem / fused: the round-1 transforms up to 2^24 cells)
+  const bool round1 = round1_requested();
+  const int p = single_term_log2(k0 + F), p2 = round1 ? fine_log2(2 * (k0 + F)) : p + 1;
   if (p2 > 24) { set_error("NUFFT (ragged): fine grid larger than 2^24 cells"); return LKB_E_UNSUPPORTED; }
+  if (!round1 && !(v2_supported(p) && v2_supported(p2))) {
+    set_error("NUFFT (ragged): fine grids of 2^%d / 2^%d cells are outside the v2 transform's range", p, p2);
+    return LKB_E_UNSUPPORTED;
+  }
   const double sigma = fmin(2.0, nufft::grid_sigma(p, k0 + F));   // (the validated rule: beta = 2.30 w from sigma = 2 on)
   const int w = kernel_width(sigma);
   const float beta = (float)nufft::es_beta(w, sigma);
@@ -1474,9 +1509,12 @@ int ls_nufft_ragged_launch(const double* d_t, const float* d_y, const int64_t* d
   nufft::gauss_legendre(GL_NQ, gl.x, gl.w);
 
   // v2 (one real transform per light curve, nufft_v2.cuh) when both fine grids are in range
-  if (fft_mode(p) == 3 && fft_mode(p2) == 3)
+  if (fft_mode(p) == 3 && fft_mode(p2) == 3) {
+    record_plan(true, p, p2);
     return ls_nufft_ragged_v2(d_t, d_y, d_off, d_po, B, ptotal, nmax, d_span, h_span, d_ysum, F, f0, df, k0, p, p2, w, beta,
                               cap_mb, normalization, d_ns, d_pow, st, 0);
+  }
+  record_plan(false, p, p2);
 
   Cad *cad = nullptr, *cad2 = nullptr;
   float2 *dec = nullptr, *dec2 = nullptr, *Za = nullptr, *Zb = nullptr, *Zw = nullptr;
@@ -1584,6 +1622,7 @@ int ls_nufft_chi2_ragged_launch(const double* d_t, const float* d_y, const int64
   const double sigma = fmin(2.0, nufft::grid_sigma(p, kmax));
   const int w = kernel_width(sigma);
   const float beta = (float)nufft::es_beta(w, sigma);
+  record_plan(true, p, p2);
   return ls_nufft_ragged_v2(d_t, d_y, d_off, d_po, B, ptotal, nmax, d_span, h_span, d_ysum, F, f0, df, k0, p, p2, w, beta,
                             ragged_cap_mb(), normalization, d_ns, d_pow, st, nterms);
 }

@@ -59,6 +59,16 @@ def ls_last_escalated():
     return int(L.load().lkb_ls_last_escalated())
 
 
+def ls_last_nufft_plan():
+    """Transform of the most recent NUFFT Lomb-Scargle call: ("v2" or "round-1", p, p2) - the flux and window-term fine
+    grids have 2^p and 2^p2 cells - or None before the first one."""
+    out = np.zeros(3, dtype=np.int32)
+    L.check(L.load().lkb_ls_last_nufft_plan(L.ptr(out)))
+    if out[0] < 0:
+        return None
+    return ("v2" if out[0] == 1 else "round-1", int(out[1]), int(out[2]))
+
+
 def profile_enable(on=True):
     """Record CUDA events around the dominant kernel of each subsequent call (see lkb200.h)."""
     L.check(L.load().lkb_profile_enable(1 if on else 0))

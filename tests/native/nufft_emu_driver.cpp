@@ -41,6 +41,7 @@ extern "C" {
 
 const char* emu_last_error() { return lkb::g_err; }
 int emu_last_escalated() { return lkb::ls_nufft_last_escalated(); }
+void emu_last_nufft_plan(int* out3) { lkb::ls_nufft_last_plan(out3); }
 
 // diagnostic: copy of a workspace slot as the last call left it (returns the slot's size in bytes)
 int64_t emu_ws_read(int slot, void* dst, int64_t bytes) {

@@ -33,7 +33,23 @@ def emu(tmp_path_factory):
                                      c_vp, c_vp]
     lib.emu_last_error.restype = ctypes.c_char_p
     lib.emu_last_escalated.restype = ctypes.c_int
+    lib.emu_last_nufft_plan.argtypes = [c_vp]
     return lib
+
+
+def _plan(emu):
+    """(transform, p, p2) of the last call: "v2" = one real transform per light curve, "round-1" = pair-packed."""
+    out = np.zeros(3, np.int32)
+    emu.emu_last_nufft_plan(out.ctypes.data)
+    return ("v2" if out[0] == 1 else "round-1", int(out[1]), int(out[2]))
+
+
+def _fine_log2(kmax):
+    """nufft_core.h fine_grid_log2 at upsampling 2: the smallest 2^p >= 4 kmax."""
+    p = 4
+    while (1 << p) < 4 * kmax:
+        p += 1
+    return p
 
 
 def _excess(got, ref):
@@ -84,7 +100,8 @@ def _shared_inputs(seed, N, F, B, oversample=5.0, k0=1):
     (3, 5.0, 1, 2, 0, {}),                                   # amplitude, one-shot, odd batch
     (4, 1.0, 1, 1, 0, {}),                                   # psd, df * baseline = 1 (wrap-around of the fine grid)
     (5, 5.0, 3, 2, 2, {}),                                   # prepare + run in chunks of 2 (two buffer sets), k0 = 3
-    (6, 5.0, 1, 2, 0, {"LKB_NUFFT_GROUP_MB": "0.05", "LKB_NUFFT_TWIDDLE_CHAIN": "1", "LKB_NUFFT_W": "10"}),
+    (6, 5.0, 1, 2, 0, {"LKB_NUFFT_FFT": "global", "LKB_NUFFT_GROUP_MB": "0.05", "LKB_NUFFT_TWIDDLE_CHAIN": "1",
+                       "LKB_NUFFT_W": "10"}),                 # round-1 global passes in groups of pairs
     (3, 5.0, 1, 2, 0, {"LKB_NUFFT_FFT": "smem"}),            # four-step transform in shared memory, one tile
     (3, 5.0, 2, 1, 2, {"LKB_NUFFT_FFT": "smem", "LKB_NUFFT_TWIDDLE_CHAIN": "1", "F": "1100", "LKB_NUFFT_TILE": "1024"}),  # 8 tiles
     (5, 1.0, 1, 2, 0, {"LKB_NUFFT_FFT": "fused", "F": "1100", "LKB_NUFFT_TILE": "1024"}),        # spreading fused in
@@ -110,6 +127,9 @@ def test_shared_grid_translation_unit_on_the_emulator(emu, monkeypatch, B, overs
             df, rot.ctypes.data, rot2.ctypes.data, F_low, normalization, scale, power.ctypes.data]
     rc = emu.emu_nufft_shared_chunked(*args, chunk) if chunk else emu.emu_nufft_shared(*args)
     assert rc == 0, emu.emu_last_error()
+    # every grid takes the v2 transform (flux grid >= 2^14 cells) unless the round-1 one is asked for by name
+    p_fine = _fine_log2(k0 + F)
+    assert _plan(emu) == (("round-1", p_fine, p_fine + 1) if "LKB_NUFFT_FFT" in env else ("v2", max(p_fine, 14), p_fine + 1))
     for b in range(B):
         p = ols.ls_slow_psd(t, Y[b], freq)
         if normalization == 2:
@@ -119,7 +139,7 @@ def test_shared_grid_translation_unit_on_the_emulator(emu, monkeypatch, B, overs
             ref = p * scale
             ex = np.abs(power[b] - ref) / (2e-5 * ref.max() + 2e-4 * ref)
         assert ex.max() < 0.5, (b, int(np.argmax(ex)), ex.max())
-    if F >= 3500 and "LKB_NUFFT_FFT" not in env:      # the v2 transform really ran: the global passes round differently
+    if "LKB_NUFFT_FFT" not in env:             # the v2 transform really ran: the round-1 global passes round differently
         monkeypatch.setenv("LKB_NUFFT_FFT", "global")
         monkeypatch.delenv("LKB_NUFFT_VERIFY", raising=False)
         power_g = np.zeros((B, F), np.float32)
@@ -147,8 +167,9 @@ def test_ragged_translation_unit_on_the_emulator(emu, monkeypatch, fft):
     """K1 layout: per-light-curve times, padded CSR, one shared regular grid; odd batch, mixed amplitudes, psd scale;
     global radix passes, the four-step shared-memory transform, and a fine-grid budget so small that the batch runs
     as three groups of one pair through the same buffers."""
-    if fft == "groups":
+    if fft == "groups":                                      # round-1 global passes, three groups of one pair
         monkeypatch.setenv("LKB_NUFFT_RAGGED_MB", "0.05")
+        monkeypatch.setenv("LKB_NUFFT_FFT", "global")
     elif fft == "v2groups":
         monkeypatch.setenv("LKB_NUFFT_RAGGED_MB", "0.9")       # 2^14 + 2^15 cells: ~0.4 MB per light curve -> groups of two
     elif fft and fft != "v2":
@@ -183,6 +204,8 @@ def test_ragged_translation_unit_on_the_emulator(emu, monkeypatch, fft):
     rc = emu.emu_nufft_ragged(tt.ctypes.data, yy.ctypes.data, off.ctypes.data, poff.ctypes.data, B, ptotal, max(ns),
                               span.ctypes.data, ysum.ctypes.data, F, f0, df, 1, scale.ctypes.data, power.ctypes.data)
     assert rc == 0, emu.emu_last_error()
+    p_fine = _fine_log2(1 + F)
+    assert _plan(emu) == (("round-1", p_fine, p_fine + 1) if fft in ("smem", "groups") else ("v2", max(p_fine, 14), max(p_fine, 14) + 1))
     for b in range(B):
         ref = ols.ls_slow_psd(times[b], fluxes[b], freq) * scale[b]
         ex = np.abs(power[b] - ref) / (2e-5 * ref.max() + 2e-4 * ref)
@@ -316,3 +339,62 @@ def test_escalation_pass_strides_over_more_light_curves_than_grid_rows(emu, monk
         worst = max(worst, float(_excess(power[b].astype(np.float64), ref).max()))
     print("worst tolerance excess over 40 escalated light curves:", worst)
     assert worst < 0.1
+
+
+def _partner_pair(seed, N, F):
+    """A quiet light curve (white noise of 1e-4 and one 3e-3 outlier, a cosmic-ray hit) and a loud one (a 3e-2
+    sinusoid at bin F / 2, almost no noise) on one cadence grid; shared grid f_k = (1 + k) df at oversample 5."""
+    rng = np.random.default_rng(seed)
+    t = np.sort(rng.uniform(0, 30.0, N))
+    trel = t - t[0]
+    df = 1.0 / (5.0 * trel[-1])
+    freq = df * (1 + np.arange(F))
+    quiet = 1 + 1e-4 * rng.normal(size=N)
+    quiet[N // 3] += 3e-3
+    loud = 1 + 3e-2 * np.sin(2 * np.pi * freq[F // 2] * t + 0.3) + 1e-7 * rng.normal(size=N)
+    return t, trel, freq, df, quiet, loud
+
+
+def _run_pair(emu, t, trel, freq, df, Y):
+    B, N, F = Y.shape[0], len(t), len(freq)
+    yc = (Y - Y.mean(axis=1, keepdims=True)).astype(np.float32)
+    Npad = ((N + 63) // 64) * 64
+    ycp = np.zeros((B, Npad), np.float32)
+    ycp[:, :N] = yc
+    ysum = ycp.astype(np.float64).sum(axis=1).astype(np.float32)
+    absmax = np.abs(ycp).max(axis=1).astype(np.float32)
+    F_low = int((freq * trel[-1] <= 2.0).sum()) + 1
+    rot, rot2 = _window_rows(trel, freq, F_low)
+    power = np.zeros((B, F), np.float32)
+    rc = emu.emu_nufft_shared(trel.ctypes.data, N, ycp.ctypes.data, Npad, ysum.ctypes.data, absmax.ctypes.data, B,
+                              freq.ctypes.data, F, freq[0], df, rot.ctypes.data, rot2.ctypes.data, F_low, 2, 1.0,
+                              power.ctypes.data)
+    assert rc == 0, emu.emu_last_error()
+    return power
+
+
+def test_small_grid_light_curve_does_not_depend_on_its_partner(emu, monkeypatch):
+    """k0 + F <= 2048 (a fine grid below 2^14 cells) used to take the round-1 transform, which packs two light curves
+    into one complex transform: the quiet one's spectrum then depended on its loud neighbour, worst next to the
+    neighbour's line.  Every single-term grid now takes the v2 transform: the quiet light curve's row is bitwise the
+    same in either order (and alone), and within the stated tolerance of the fp64 oracle on every bin.  The round-1
+    transform, still reachable by name, shows the dependence the default path must not have (1.2x the tolerance next to
+    the partner's line, 1.9x in the other order)."""
+    monkeypatch.setenv("LKB_NUFFT_ESCALATE", "0")         # the transform itself, not the double-precision second pass
+    N, F = 6000, 1000
+    t, trel, freq, df, quiet, loud = _partner_pair(3, N, F)
+    ref = np.sqrt(ols.ls_slow_psd(t, quiet, freq)) * np.sqrt(4.0 / N)          # amplitude
+    a = _run_pair(emu, t, trel, freq, df, np.stack([quiet, loud]))
+    assert _plan(emu) == ("v2", 14, 13)
+    b = _run_pair(emu, t, trel, freq, df, np.stack([loud, quiet]))
+    alone = _run_pair(emu, t, trel, freq, df, quiet[None, :])
+    assert np.array_equal(a[0], b[1]) and np.array_equal(a[0], alone[0])
+    ex = _excess(a[0].astype(np.float64), ref)
+    monkeypatch.setenv("LKB_NUFFT_FFT", "global")
+    a1 = _run_pair(emu, t, trel, freq, df, np.stack([quiet, loud]))
+    assert _plan(emu) == ("round-1", 12, 13)
+    ex1 = _excess(a1[0].astype(np.float64), ref)
+    print("quiet light curve next to a loud one, worst excess over the tolerance: v2 %.3g, round-1 %.3g (bin %d)"
+          % (ex.max(), ex1.max(), int(np.argmax(ex1))))
+    assert ex.max() < 0.1
+    assert ex1.max() > 1.0
