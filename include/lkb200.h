@@ -229,6 +229,21 @@ int lkb_regress(const double* X, int x_batched, const double* y, const double* f
                 double* coeff, double* model, uint8_t* outlier_mask, int32_t* status_out, double* coeff_cov,
                 int mem, void* stream);
 
+/* lkb_regress with two more arguments (lkb_regress is lkb_regress_ex(..., 0, 0), bitwise):
+ *   prior_batched  0: prior_mu / prior_sigma are [K] (shared); 1: they are [B, K], one prior per light curve
+ *                  (CBVCorrector.correct gives each light curve its own width median(flux_err) / sqrt(|alpha_b|))
+ *   flags          LKB_REGRESS_EXACT_INVARIANT: each light curve's outputs are bitwise independent of B and of the
+ *                  other light curves of the call, and equal for a shared and a batched X - the exact fp64 Gram
+ *                  kernels only (never the tcgen05 Gram), per-light-curve model kernels (never the batched model
+ *                  GEMM), the Gram split over CTAs decided by N alone.  For callers that compare results across calls
+ *                  of different batches, such as the alpha optimiser of CBVCorrector.correct_batch. */
+#define LKB_REGRESS_EXACT_INVARIANT 1
+int lkb_regress_ex(const double* X, int x_batched, const double* y, const double* flux_err,
+                   const uint8_t* cadence_mask, const double* prior_mu, const double* prior_sigma,
+                   int B, int64_t N, int K, double clip_sigma, int niters,
+                   double* coeff, double* model, uint8_t* outlier_mask, int32_t* status_out, double* coeff_cov,
+                   int mem, void* stream, int prior_batched, int flags);
+
 /* ---- batched order statistics (K6) ---------------------------------------- */
 /* nanmedian and nanstd (ddof=0) per light curve: np.nanmedian / np.nanstd as used by
  * normalize (lightcurve.py:1253-1254) and flatten (:1003-1005). out_median/out_std [B]. */
@@ -279,6 +294,36 @@ int lkb_elasticnet(const double* X, int x_batched, const double* y, const uint8_
 int lkb_acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets,
                     const int64_t* win_start, const int64_t* win_len, double* metric, double* acf,
                     int mem, void* stream);
+
+/* ---- CBVCorrector goodness metrics (K9) ---------------------------------- */
+/* The under-fitting metric of metrics.py:178-255 (underfit_metric_neighbors with _compute_correlation) for B targets
+ * whose neighbours are rows of one pool:
+ *   pool        [P, G] fp64: neighbour fluxes on a common cadence grid (NaN where a neighbour has no cadence)
+ *   target      [B, G] fp64: target fluxes on the same grid (NaN where absent or left out by the cadence mask)
+ *   nb_offsets  [B + 1] int64, nb_index [nb_offsets[B]] int32: HOST CSR of each target's neighbours (pool rows)
+ *   metric      [B]: drop every cadence where the target or any of its neighbours is NaN; correlation with each
+ *               neighbour over the rest (RMS 0 read as inf); 2 / (1 + exp(scale * nanmean(|c_i|^3, with the zeroed
+ *               diagonal: divide by M + 1))), scale = log(2 / 0.95 - 1) / (0.0007 + 0.8083 n^-0.5023)
+ *   n_used      [B] int32 (nullable): the cadences used;  c3_mean [B] (nullable): that nanmean of |c_i|^3
+ * pool, target and the outputs follow `mem`; the call returns once the stream has consumed the host CSR.
+ * LKB_E_ARG for an index outside the pool, LKB_E_UNSUPPORTED when the cadence mask and neighbour list of one target do
+ * not fit in shared memory (227 KB: G / 8 + 20 M bytes). */
+int lkb_underfit_metric(const double* pool, int P, const double* target, int B, int64_t G, const int64_t* nb_offsets,
+                        const int32_t* nb_index, double* metric, int32_t* n_used, double* c3_mean, int mem,
+                        void* stream);
+
+/* The per-light-curve terms of the over-fitting metric (metrics.py:23-123) from fp32 Lomb-Scargle power rows, as the
+ * LS entries write them:
+ *   corrected, original  power of the corrected and the original light curve; light curve b's row at offsets[b]
+ *                        (HOST CSR [B + 1]) or, with offsets NULL, at b * F (one shared grid of F bins)
+ *   noise                S white-noise power rows per light curve: row s of light curve b at S offsets[b] + s len_b
+ *   n_positive [B] int32  #{corrected - original > 0} (differences in fp64; NaN differences dropped)
+ *   sum_positive [B]      the sum of those differences
+ *   noise_mean [B, S]     np.nanmean of each noise row
+ * The host turns them into the metric: 2 / (1 + exp(max(mean_s sum_positive / (n_positive noise_mean[s]), 0))). */
+int lkb_overfit_terms(const float* corrected, const float* original, const float* noise, const int64_t* offsets, int B,
+                      int64_t F, int S, int32_t* n_positive, double* sum_positive, double* noise_mean, int mem,
+                      void* stream);
 
 /* ---- multi-GPU: the one exchange step of the path (SURVEY.md 8e) ------------------ */
 /* A LightCurveCollection is sharded BY TARGET over one process per GPU; the only data exchange is the

@@ -20,6 +20,7 @@ LS_NORM_PSD_RAW, LS_NORM_PSD_SCALE, LS_NORM_AMPLITUDE = 0, 1, 2
 LS_ALGO_AUTO, LS_ALGO_SIMT, LS_ALGO_TCGEN05, LS_ALGO_NUFFT = 0, 1, 2, 3
 FLATTEN_PATH_V2_MOMENTS, FLATTEN_PATH_V2_DIRECT, FLATTEN_PATH_V1, FLATTEN_PATH_V1_RERUN = 0, 1, 2, 3
 BLS_LIKELIHOOD, BLS_SNR = 0, 1
+REGRESS_EXACT_INVARIANT = 1
 
 c_int, c_i64, c_dbl, c_vp = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
 
@@ -58,6 +59,10 @@ SIGNATURES = {
     "lkb_flatten_last_path": (c_int, []),
     "lkb_regress": (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_dbl, c_int,
                             c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
+    "lkb_regress_ex": (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_dbl, c_int,
+                               c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int]),
+    "lkb_underfit_metric": (c_int, [c_vp, c_int, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
+    "lkb_overfit_terms": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_elasticnet": (c_int, [c_vp, c_int, c_vp, c_vp, c_int, c_i64, c_int, c_dbl, c_dbl, c_int, c_dbl, c_int,
                                c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_savgol_tables": (c_int, [c_int, c_int, c_vp, c_vp]),

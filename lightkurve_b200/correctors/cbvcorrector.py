@@ -4,10 +4,12 @@ Lomb-Scargle over-fitting metric (K1) inside a bounded scalar optimiser (SURVEY.
 
 Scope: everything that runs from arrays - the basis-vector container (`to_designmatrix`, `align`, `interpolate`),
 `correct_gaussian_prior`, the `correct` optimiser over the regularisation `alpha`, `over_fitting_metric`,
-`correct_regressioncorrector`, and `correct_elasticnet` (scikit-learn's elastic-net coordinate descent, K8; with
-`correct_elasticnet_batch` for many correctors in one call).  Out of scope here: reading CBV FITS files / downloading
-them from MAST (`load_kepler_cbvs`, `load_tess_cbvs`), the under-fitting metric (it needs a MAST search of
-neighbouring targets) and the plots.  Basis vectors are
+`under_fitting_metric` (with the neighbouring light curves handed over), `correct_regressioncorrector`,
+`correct_elasticnet` (scikit-learn's elastic-net coordinate descent, K8; with `correct_elasticnet_batch` for many
+correctors in one call) and `correct_batch` (the alpha optimiser with both goodness metrics for many correctors, the
+batch serving as its own neighbourhood; K5 + K1 + K9 per round).  Out of scope here: reading CBV FITS files /
+downloading them from MAST (`load_kepler_cbvs`, `load_tess_cbvs`), the MAST neighbour search and the plots.  Basis
+vectors are
 therefore handed over explicitly (``CBVCorrector(lc, cbvs=[...])``, an extension of the reference signature) or
 left out (``do_not_load_cbvs=True`` with an external design matrix, as in the reference's own non-remote test).
 """
@@ -23,7 +25,9 @@ from .. import units as u
 from ..lightcurve import LightCurve
 from ..units import Quantity, Time
 from .designmatrix import DesignMatrix, DesignMatrixCollection
-from .metrics import overfit_metric_lombscargle
+from .metrics import (MAST_MESSAGE, _cadence_grid, _centred, _neighbor_rows, _overfit_from_terms,
+                      _require_cadenceno, overfit_metric_lombscargle, underfit_metric_neighbors)
+from .optimize import minimize_bounded_lockstep
 from .regressioncorrector import RegressionCorrector
 
 log = logging.getLogger(__name__)
@@ -66,6 +70,70 @@ def _elasticnet_options(kwargs):
             raise TypeError("correct_elasticnet() got an unexpected keyword argument {!r}".format(key))
     opts["positive"] = bool(opts["positive"])
     return opts
+
+
+# Largest neighbour search radius (arcsec): the diagonal of a TESS camera (two CCDs wide, 24 degrees) or of one
+# Kepler / K2 CCD (cbvcorrector.py:608-617)
+_MAX_RADIUS = {"TESS": np.sqrt(2) * (86400 / 2.0), "Kepler": np.sqrt(2) * 4096, "K2": np.sqrt(2) * 4096}
+_NOT_ENOUGH = "Not enough neighboring targets were found. under_fitting_metric failed"
+# Lomb-Scargle work (cadences x bins) from which the library's `auto` takes the non-uniform FFT for one light curve
+# (lkb_ls_power, ls.cu); correct_batch applies it per light curve so that the batch does not choose the family
+_LS_NUFFT_MIN_WORK = 2.5e7
+
+
+def _separation_arcsec(ra0, dec0, ra, dec):
+    """Great-circle separation (Vincenty formula, as astropy's `SkyCoord.separation`) of degrees, in arcsec."""
+    l0, b0, l1, b1 = np.radians(ra0), np.radians(dec0), np.radians(ra), np.radians(dec)
+    dl = l1 - l0
+    num = np.hypot(np.cos(b1) * np.sin(dl), np.cos(b0) * np.sin(b1) - np.sin(b0) * np.cos(b1) * np.cos(dl))
+    den = np.sin(b0) * np.sin(b1) + np.cos(b0) * np.cos(b1) * np.cos(dl)
+    return np.degrees(np.arctan2(num, den)) * 3600.0
+
+
+def _sky(lc):
+    ra, dec = lc.meta.get("RA"), lc.meta.get("DEC")
+    if ra is None or dec is None:
+        raise ValueError("selecting neighbours by radius needs meta['RA'] and meta['DEC'] (degrees) on every light "
+                         "curve; pass `neighbor_index` to skip the sky geometry")
+    return float(ra), float(dec)
+
+
+def _own_entries(lc, pool):
+    """Pool entries that are `lc` itself: the same object or the same (known) TARGETID."""
+    tid = lc.meta.get("TARGETID")
+    return {i for i, p in enumerate(pool) if p is lc or (tid is not None and p.meta.get("TARGETID") == tid)}
+
+
+def _select_neighbors(lc, pool, exclude, radius=None, min_targets=30, max_targets=50, neighbor_index=None,
+                      coords=None):
+    """Indices into `pool` of the neighbours of `lc` by the reference's radius loop (cbvcorrector.py:586-637): the
+    nearest `max_targets` within the radius (default 5000 arcsec for TESS, 1000 for Kepler / K2), the radius growing
+    by 1.5 until `min_targets` are found or it passes the CCD diagonal.  `neighbor_index`: the candidates in order of
+    preference, instead of the sky geometry."""
+    mission = lc.meta.get("MISSION")
+    if radius is None:
+        radius = 5000 if mission == "TESS" else 1000
+    if mission not in _MAX_RADIUS:
+        raise Exception("Unknown mission")
+    if neighbor_index is not None:
+        cand = [int(i) for i in neighbor_index if int(i) not in exclude]
+        if len(cand) < min_targets:
+            raise Exception(_NOT_ENOUGH)
+        return cand[:max_targets]
+    ra0, dec0 = _sky(lc)
+    if coords is None:
+        coords = np.array([_sky(p) for p in pool]).reshape(-1, 2)
+    others = [i for i in range(len(pool)) if i not in exclude]
+    sep = _separation_arcsec(ra0, dec0, coords[others, 0], coords[others, 1])
+    order = np.argsort(sep, kind="stable")
+    r = radius
+    while True:
+        sel = [others[k] for k in order if sep[k] <= r]
+        if len(sel) >= min_targets:
+            return sel[:max_targets]
+        if r > _MAX_RADIUS[mission]:
+            raise Exception(_NOT_ENOUGH)
+        r *= 1.5
 
 
 def _per_item(value, n):
@@ -350,10 +418,22 @@ class CBVCorrector(RegressionCorrector):
                 c.alpha = alpha
 
     def correct(self, cbv_type=["SingleScale"], cbv_indices=[np.arange(1, 9)], ext_dm=None, cadence_mask=None,
-                alpha_bounds=[1e-4, 1e4], target_over_score=0.5, target_under_score=0.5, max_iter=100):
+                alpha_bounds=[1e-4, 1e4], target_over_score=0.5, target_under_score=0.5, max_iter=100,
+                neighbors=None):
         """Optimise `alpha` with a bounded scalar minimiser against the goodness metrics (cbvcorrector.py:397-501).
-        Only the over-fitting metric exists in this build: `target_under_score` must be 0 (the under-fitting metric
-        needs neighbouring targets from MAST)."""
+        The under-fitting metric needs the neighbouring light curves (`neighbors`, in place of the reference's MAST
+        search); with them and `target_under_score > 0` this is `correct_batch([self], ..., neighbors=neighbors)`.
+        Without them `target_under_score` must be 0."""
+        if neighbors is not None and target_under_score > 0:
+            CBVCorrector.correct_batch([self], cbv_type=cbv_type, cbv_indices=cbv_indices, ext_dm=ext_dm,
+                                       cadence_mask=cadence_mask, alpha_bounds=alpha_bounds,
+                                       target_over_score=target_over_score, target_under_score=target_under_score,
+                                       max_iter=max_iter, neighbors=neighbors)
+            if target_over_score > 0:
+                print("Optimized Over-fitting metric: {}".format(self.over_fitting_score))
+            print("Optimized Under-fitting metric: {}".format(self.under_fitting_score))
+            print("Optimized Alpha: {0:2.3e}".format(self.alpha))
+            return self.corrected_lc
         self._correct_initialization(cbv_type=cbv_type, cbv_indices=cbv_indices, ext_dm=ext_dm)
         if target_under_score > 0:
             raise NotImplementedError("the under-fitting metric needs a MAST search of neighbouring targets, which is "
@@ -382,9 +462,71 @@ class CBVCorrector(RegressionCorrector):
         return overfit_metric_lombscargle(self.lc.copy()[self.cadence_mask], self.corrected_lc.copy()[self.cadence_mask],
                                           n_samples=n_samples)
 
-    def under_fitting_metric(self, *args, **kwargs):
-        raise NotImplementedError("the under-fitting metric needs a MAST search of neighbouring targets "
-                                  "(outside the scope of lightkurve_b200)")
+    def under_fitting_metric(self, neighbors=None, radius=None, min_targets=30, max_targets=50, neighbor_index=None):
+        """`metrics.underfit_metric_neighbors` of the corrected light curve on the used cadences, its neighbours picked
+        from `neighbors` (a list or `LightCurveCollection`, in place of the reference's MAST search) by the reference's
+        radius loop (cbvcorrector.py:586-637) on great-circle separations from meta["RA"], meta["DEC"] (degrees).  A
+        light curve is never its own neighbour.  `neighbor_index`: indices into `neighbors` in order of preference,
+        instead of the sky geometry.  `coords`: the pool's [P, 2] (RA, DEC), when the caller has them already."""
+        if self.corrected_lc is None:
+            raise Exception("A corrected light curve does not exist, please run correct first")
+        if neighbors is None:
+            raise NotImplementedError(MAST_MESSAGE)
+        pool = list(neighbors)
+        sel = _select_neighbors(self.lc, pool, _own_entries(self.lc, pool), radius, min_targets, max_targets,
+                                neighbor_index)
+        corrected = self.corrected_lc.copy()[self.cadence_mask]
+        return underfit_metric_neighbors(corrected, min_targets=min_targets, max_targets=max_targets,
+                                         interpolate=self.interpolated_cbvs, extrapolate=self.extrapolated_cbvs,
+                                         neighbors=[pool[i] for i in sel])
+
+    @staticmethod
+    def correct_batch(correctors, cbv_type=["SingleScale"], cbv_indices=[np.arange(1, 9)], ext_dm=None,
+                      cadence_mask=None, alpha_bounds=[1e-4, 1e4], target_over_score=0.5, target_under_score=0.5,
+                      max_iter=100, neighbors=None, radius=None, min_targets=30, max_targets=50, neighbor_index=None):
+        """`correct` for many correctors, the minimisers of all correctors run in lock step: each round fits every
+        still-active corrector with its own prior width in one regression call (bitwise independent of the batch,
+        LKB_REGRESS_EXACT_INVARIANT), computes their corrected and white-noise periodograms on each corrector's
+        original-periodogram grid (with the kernel family the corrector's own call would take), and both goodness
+        metrics in one K9 call each.  The inputs stay on the GPU across rounds.  Every corrector ends in the state its
+        own `correct` would leave (`alpha`, corrected / model / diagnostic light curves, `coefficients`,
+        `cadence_mask`, `over_fitting_score` at n_samples=10, `under_fitting_score`) and gains `optimization_trace`:
+        one (alpha, over, under, mean_noise_power, n_positive, sum_positive) per evaluation of its objective.
+
+        Neighbours for the under-fitting metric come from `neighbors` or, by default, from the batch's own light
+        curves (the other targets of the same CCD and sector, which is what the reference's MAST search returns),
+        selected per corrector as in `under_fitting_metric` (`radius`, `min_targets`, `max_targets`,
+        `neighbor_index`: one index list per corrector).  Correctors built with `interpolate_cbvs=True` raise
+        NotImplementedError here: their neighbours would have to be interpolated pair by pair.
+
+        `ext_dm` and `cadence_mask` are shared or lists with one entry per corrector.  White noise: one
+        ``np.random.randn(n_cadences, 1)`` per active corrector per round, in batch order, from numpy's global stream,
+        then the final re-fit's draws and the ten of each final over-fitting score, corrector by corrector - a batch
+        of one consumes exactly the draws of the reference's `correct`.  Returns the corrected light curves."""
+        correctors = list(correctors)
+        B = len(correctors)
+        ext = ext_dm if _per_item(ext_dm, B) else [ext_dm] * B
+        masks = cadence_mask if _per_item(cadence_mask, B) else [cadence_mask] * B
+        for c, e, m in zip(correctors, ext, masks):
+            # a copy per corrector: the prior widths set on the design matrices differ from corrector to corrector
+            c._correct_initialization(cbv_type=cbv_type, cbv_indices=cbv_indices,
+                                      ext_dm=None if e is None else copy.deepcopy(e))
+            c.optimization_params = {"alpha_bounds": alpha_bounds, "target_over_score": target_over_score,
+                                     "target_under_score": target_under_score, "max_iter": max_iter,
+                                     "cadence_mask": m, "over_metric_nSamples": 1}
+            c.optimization_trace = []
+        run = _GoodnessBatch(correctors, masks, target_over_score, target_under_score)
+        if target_under_score > 0:
+            run.set_neighbors(neighbors, radius, min_targets, max_targets, neighbor_index)
+        results = minimize_bounded_lockstep(run.evaluate, [alpha_bounds] * B, maxiter=max_iter)
+        xs = np.array([r.x for r in results])
+        run.evaluate(np.arange(B), xs, record=False, finish=True)   # the minimiser does not end on its best point
+        for b, c in enumerate(correctors):
+            c._set_prior_width(np.median(c.lc.flux_err.value) / np.sqrt(np.abs(xs[b])))
+            c.over_fitting_score = c.over_fitting_metric(n_samples=10) if target_over_score > 0 else -1.0
+            c.under_fitting_score = float(run.under[b]) if target_under_score > 0 else -1.0
+            c.alpha = results[b].x
+        return [c.corrected_lc for c in correctors]
 
     def _goodness_metric_obj_fun(self, alpha):
         """Penalty = -(over metric), saturating (1 % leak) above the target (cbvcorrector.py:781-854)."""
@@ -405,3 +547,267 @@ class CBVCorrector(RegressionCorrector):
             kinds = ", ".join(str(c.cbv_type) for c in self.cbvs)
             return "CBVCorrector (ID: {}, CBVs: {})".format(self.lc.targetid, kinds)
         return "CBVCorrector (ID: {}, no CBVs)".format(self.lc.targetid)
+
+
+def _use_device():
+    """Whether correct_batch keeps its inputs on the GPU (CUDA torch tensors, device-mode engine calls)."""
+    try:
+        import torch
+    except ImportError:
+        return False
+    return torch.cuda.is_available()
+
+
+def _morton(ra, dec):
+    """Z-order key of sky positions: targets close on the sky get close keys."""
+    x = np.clip(np.asarray(ra, dtype=np.float64) / 360.0 * 65535, 0, 65535).astype(np.uint64)
+    y = np.clip((np.asarray(dec, dtype=np.float64) + 90.0) / 180.0 * 65535, 0, 65535).astype(np.uint64)
+    key = np.zeros_like(x)
+    for bit in range(16):
+        key |= ((x >> np.uint64(bit)) & np.uint64(1)) << np.uint64(2 * bit)
+        key |= ((y >> np.uint64(bit)) & np.uint64(1)) << np.uint64(2 * bit + 1)
+    return key
+
+
+class _GoodnessBatch:
+    """The objective of CBVCorrector.correct for a set of correctors, one round at a time: the regression with
+    per-corrector priors, the over-fitting metric (K1 periodograms + lkb_overfit_terms) and the under-fitting metric
+    (lkb_underfit_metric), as in _goodness_metric_obj_fun (cbvcorrector.py:781-854).
+
+    The design matrices, fluxes, flux errors and cadence masks (per design-matrix shape), the original periodograms
+    and the neighbour pool go to the device once and stay there; a round gathers the rows of its active correctors
+    there.  Per round the models come back (the normalisation by each corrected light curve's median and the white
+    noise, drawn from numpy's global stream, are host work on arrays) and the corrected rows, the noise rows and the
+    under-fitting target rows go up; the power rows never leave the device.  Corrector state (light curves,
+    diagnostics) is built once, at the final re-fit."""
+
+    def __init__(self, correctors, masks, target_over, target_under):
+        self.dev = _use_device()
+        self.cs = correctors
+        self.target_over, self.target_under = target_over, target_under
+        B = len(correctors)
+        self.masks, self.flux, self.fe_used, self.time_used, self.sigma0 = [], [], [], [], []
+        for c, m in zip(correctors, masks):
+            n = len(c.lc.flux)
+            m = np.ones(n, bool) if m is None else np.asarray(m, dtype=bool)
+            if m.shape != (n,):
+                raise ValueError("cadence_mask must have one entry per cadence")
+            self.masks.append(m)
+            fe = np.asarray(c.lc.flux_err.value, dtype=np.float64)
+            self.flux.append(np.asarray(c.lc.flux.value, dtype=np.float64))
+            self.fe_used.append(((fe ** 2 + 0.0 ** 2) ** 0.5)[m])           # the corrected light curve's flux_err
+            self.time_used.append(np.asarray(c.lc.time.value, dtype=np.float64)[m])
+            self.sigma0.append(np.median(c.lc.flux_err.value))
+        self.groups = []
+        by_shape = {}
+        for b, c in enumerate(correctors):
+            X = RegressionCorrector._dense_X(c.design_matrix_collection)
+            by_shape.setdefault(X.shape, []).append((b, X))
+        for shape, items in by_shape.items():
+            members = [b for b, _ in items]
+            Xs = [X for _, X in items]
+            shared = all(X is Xs[0] or np.array_equal(X, Xs[0]) for X in Xs)
+            FE = np.stack([np.asarray(correctors[b].lc.flux_err.value, dtype=np.float64) for b in members])
+            allnan = np.all(~np.isfinite(FE), axis=1)
+            self.groups.append(dict(
+                members=members, set=set(members), pos={b: j for j, b in enumerate(members)}, K=shape[1],
+                shared=shared, X=self.up(Xs[0] if shared else np.stack(Xs)),
+                Y=self.up(np.stack([self.flux[b] for b in members])),
+                FE=None if allnan.all() else self.up(np.where(allnan[:, None], 1.0, FE)),
+                CM=self.up(np.stack([self.masks[b] for b in members]).astype(np.uint8)),
+                PM=np.stack([np.asarray(correctors[b].design_matrix_collection.prior_mu, dtype=np.float64)
+                             for b in members])))
+        self.under = np.full(B, np.nan)
+        self.cta_order = None
+        if target_over > 0:
+            self._setup_periodograms()
+
+    # ---- host numpy or device tensors, one code path ----
+    def up(self, a):
+        a = np.ascontiguousarray(a)
+        if not self.dev:
+            return a
+        import torch
+        return torch.from_numpy(a).cuda()
+
+    def down(self, a):
+        return a.cpu().numpy() if self.dev else np.asarray(a)
+
+    def take(self, a, rows):
+        """Rows `rows` (host int array, or None for all) of a resident array."""
+        if rows is None or a is None:
+            return a
+        if self.dev:
+            import torch
+            return a.index_select(0, torch.from_numpy(np.asarray(rows, dtype=np.int64)).cuda())
+        return np.ascontiguousarray(a[rows])
+
+    def _setup_periodograms(self):
+        """The original light curve's periodogram of each corrector, once: its grid serves every later periodogram.
+        Correctors with the same grid and kernel family form one periodogram group, whose original power rows stay
+        resident."""
+        from ..periodogram import _PER_DAY, LombScarglePeriodogram
+        self.pg, self.ls_groups = [], {}
+        orig_rows = {}
+        for b, (c, m) in enumerate(zip(self.cs, self.masks)):
+            orig, oflux = _centred(c.lc.copy()[m])
+            prep = LombScarglePeriodogram._prepare(orig)
+            freq = np.asarray(prep["frequency"].to(_PER_DAY).value, dtype=np.float64)
+            t = np.asarray(prep["time"], dtype=np.float64)
+            # the family the corrector's own call would take (never decided from the batch)
+            fam = "nufft" if len(t) * len(freq) >= _LS_NUFFT_MIN_WORK else "direct"
+            key = (freq.tobytes(), fam)
+            g = self.ls_groups.setdefault(key, dict(members=[], freq=freq, fam=fam))
+            self.pg.append(dict(time=t, key=key, row=len(g["members"])))
+            g["members"].append(b)
+            orig_rows[b] = (t, oflux)
+        for key, g in self.ls_groups.items():
+            g["freq_dev"] = self.up(g["freq"])
+            g["orig"] = self._power(g, [orig_rows[b] for b in g["members"]])
+
+    def _power(self, g, rows):
+        """float32 amplitude power [len(rows), F] of (time, flux) rows on the group's grid (device or host)."""
+        from .. import engine
+        times, fluxes = [r[0] for r in rows], [r[1] for r in rows]
+        algos = [g["fam"], "direct"] if g["fam"] == "nufft" else ["direct"]
+        for k, algo in enumerate(algos):
+            try:
+                if not self.dev:
+                    return np.asarray(engine.ls_power_ragged(times, fluxes, g["freq"], "amplitude", None, algo=algo),
+                                      dtype=np.float32)
+                off = np.zeros(len(rows) + 1, np.int64)
+                off[1:] = np.cumsum([len(t) for t in times])
+                return engine.ls_power_ragged_device(self.up(np.concatenate(times)), self.up(np.concatenate(fluxes)),
+                                                     off, g["freq_dev"], "amplitude", None, algo=algo)
+            except Exception as e:
+                # LKB_E_UNSUPPORTED from the non-uniform FFT (unsorted times, too few cadences): the direct sums, as
+                # the library's `auto` does for a light curve that does not qualify
+                if k + 1 == len(algos) or getattr(e, "status", None) != -5:
+                    raise
+
+    def set_neighbors(self, neighbors, radius, min_targets, max_targets, neighbor_index):
+        cs = self.cs
+        if any(c.interpolated_cbvs for c in cs):
+            raise NotImplementedError("correct_batch cannot compute the under-fitting metric of correctors built with "
+                                      "interpolate_cbvs=True: their neighbours would be interpolated pair by pair")
+        default = neighbors is None
+        pool = [c.lc for c in cs] if default else list(neighbors)
+        if neighbor_index is not None and len(neighbor_index) != len(cs):
+            raise ValueError("neighbor_index needs one index list per corrector")
+        coords = None
+        if neighbor_index is None:
+            coords = np.array([_sky(p) for p in pool]).reshape(-1, 2)
+        sel = []
+        for b, c in enumerate(cs):
+            excl = _own_entries(c.lc, pool) | ({b} if default else set())
+            sel.append(_select_neighbors(c.lc, pool, excl, radius, min_targets, max_targets,
+                                         None if neighbor_index is None else neighbor_index[b], coords))
+        used = sorted({i for s in sel for i in s})
+        for c in cs:
+            _require_cadenceno(c.lc)
+        for p in used:
+            _require_cadenceno(pool[p])
+        if coords is not None:
+            # pool rows and target CTAs in sky (Z-) order: targets that share neighbours run in the same CTA wave and
+            # re-read those rows from L2.  The kernel's results do not depend on the order.
+            used = [used[k] for k in np.argsort(_morton(coords[used, 0], coords[used, 1]), kind="stable")]
+            own = np.array([_sky(c.lc) for c in cs]).reshape(-1, 2)
+            self.cta_order = np.argsort(_morton(own[:, 0], own[:, 1]), kind="stable")
+        row_of = {p: r for r, p in enumerate(used)}
+        self.c0, self.G = _cadence_grid([np.asarray(c.lc.cadenceno)[m] for c, m in zip(cs, self.masks)])
+        self.pool = self.up(_neighbor_rows([pool[p] for p in used], None, None, self.c0, self.G))
+        self.pos_on_grid = [np.asarray(c.lc.cadenceno, dtype=np.int64)[m] - self.c0 for c, m in zip(cs, self.masks)]
+        self.nb = [np.array([row_of[i] for i in s], dtype=np.int32) for s in sel]
+
+    def _centred(self, b, model):
+        """The corrected light curve on its used cadences, ``remove_nans().normalize() - 1`` (metrics._centred on
+        arrays): (kept cadences, centred flux, mean normalised flux_err)."""
+        f = self.flux[b][self.masks[b]] - model[self.masks[b]]
+        keep = ~np.isnan(f)
+        if not keep.all():
+            f = f[keep]
+        med = np.median(f)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return keep, f / med - 1.0, np.nanmean(self.fe_used[b][keep] / med)
+
+    def evaluate(self, idx, alphas, record=True, finish=False):
+        from .. import engine
+        idx = np.asarray(idx)
+        cs = self.cs
+        pos = {b: k for k, b in enumerate(idx)}
+        models = {}
+        # regression: every corrector its own prior width, results independent of the batch
+        for g in self.groups:
+            act = [b for b in idx if b in g["set"]]
+            if not act:
+                continue
+            rows = None if len(act) == len(g["members"]) else [g["pos"][b] for b in act]
+            ps = np.stack([np.ones(g["K"]) * (self.sigma0[b] / np.sqrt(np.abs(alphas[pos[b]]))) for b in act])
+            pm = g["PM"] if rows is None else g["PM"][rows]
+            res = engine.regress(g["X"] if g["shared"] else self.take(g["X"], rows), self.take(g["Y"], rows),
+                                 self.take(g["FE"], rows), self.take(g["CM"], rows), self.up(pm), self.up(ps),
+                                 exact_invariant=True)
+            status = self.down(res["status"])
+            if np.any(status != 0):
+                raise np.linalg.LinAlgError("Singular matrix")
+            model = self.down(res["model"])
+            if finish:
+                coeff, om = self.down(res["coefficients"]), self.down(res["outlier_mask"]).astype(bool)
+            for j, b in enumerate(act):
+                models[b] = model[j]
+                if finish:
+                    c = cs[b]
+                    c.cadence_mask = self.masks[b]
+                    c.outlier_mask = om[j]
+                    c.coefficients = coeff[j]
+                    c.coefficients_err = np.zeros(len(c.coefficients)) * np.nan
+                    c._finish(model[j])
+        n = len(idx)
+        cen = {b: self._centred(b, models[b]) for b in idx}
+        over, under = np.ones(n), np.ones(n)
+        npos, spos, nmean = np.zeros(n, np.int64), np.full(n, np.nan), np.full(n, np.nan)
+        if self.target_over > 0:
+            noise = {}
+            for b in idx:                                     # numpy's global stream, in batch order
+                noise[b] = (np.random.randn(len(self.pg[b]["time"]), 1) * cen[b][2]).T[0]
+            for key, g in self.ls_groups.items():
+                act = [b for b in idx if self.pg[b]["key"] == key]
+                if not act:
+                    continue
+                rows = [(self.time_used[b][cen[b][0]], cen[b][1]) for b in act] + \
+                       [(self.pg[b]["time"], noise[b]) for b in act]
+                pw = self._power(g, rows)
+                m = len(act)
+                orig = g["orig"] if m == len(g["members"]) else self.take(g["orig"], [self.pg[b]["row"] for b in act])
+                terms = {name: self.down(v) for name, v in engine.overfit_terms(pw[:m], orig, pw[m:], None, 1).items()}
+                for j, b in enumerate(act):
+                    k = pos[b]
+                    npos[k] = int(terms["n_positive"][j])
+                    spos[k] = float(terms["sum_positive"][j])
+                    nmean[k] = float(terms["noise_mean"][j, 0])
+                    over[k] = _overfit_from_terms(npos[k], spos[k], [nmean[k]])
+        if self.target_under > 0:
+            order = idx if self.cta_order is None else np.array([b for b in self.cta_order if b in pos])
+            T = np.full((n, self.G), np.nan)
+            for r, b in enumerate(order):
+                keep, cflux, _ = cen[b]
+                T[r, self.pos_on_grid[b][keep]] = cflux
+            off = np.zeros(n + 1, np.int64)
+            off[1:] = np.cumsum([len(self.nb[b]) for b in order])
+            met = self.down(engine.underfit_metric(self.pool, self.up(T), off,
+                                                   np.concatenate([self.nb[b] for b in order]))["metric"])
+            for r, b in enumerate(order):
+                under[pos[b]] = met[r]
+            self.under[idx] = under
+        pen = np.empty(n)
+        for k, b in enumerate(idx):
+            o, un = over[k], under[k]
+            if record:
+                cs[b].optimization_trace.append((float(alphas[k]), float(o), float(un), float(nmean[k]), int(npos[k]),
+                                                 float(spos[k])))
+            if self.target_over > 0 and o >= self.target_over:
+                o = self.target_over + 0.01 * (o - self.target_over)
+            if self.target_under > 0 and un >= self.target_under:
+                un = self.target_under + 0.01 * (un - self.target_under)
+            pen[k] = -(o + un)
+        return pen

@@ -219,7 +219,7 @@ int bls_bin_index(const double*, int64_t, double, double, double, int32_t*, int,
 int flatten(const double*, const double*, const double*, const uint8_t*, const int64_t*, int, int, int, double, int,
             double, double*, double*, double*, int, cudaStream_t);
 int regress(const double*, int, const double*, const double*, const uint8_t*, const double*, const double*, int,
-            int64_t, int, double, int, double*, double*, uint8_t*, int32_t*, double*, int, cudaStream_t);
+            int64_t, int, double, int, double*, double*, uint8_t*, int32_t*, double*, int, cudaStream_t, int, int);
 int elasticnet(const double*, int, const double*, const uint8_t*, int, int64_t, int, double, double, int, double, int,
                double*, double*, int32_t*, double*, uint8_t*, int, cudaStream_t);
 int nanmedian_std(const double*, const int64_t*, int, double*, double*, int, cudaStream_t);
@@ -227,6 +227,10 @@ int pg_logmedian(const double*, int, int64_t, const int32_t*, const int32_t*, in
 int acf_windows(const double*, const int64_t*, int, const int64_t*, const int64_t*, const int64_t*, double*, double*,
                 int, cudaStream_t);
 int savgol_tables_host(int, int, double*, double*);
+int underfit_metric(const double*, int, const double*, int, int64_t, const int64_t*, const int32_t*, double*, int32_t*,
+                    double*, int, cudaStream_t);
+int overfit_terms(const float*, const float*, const float*, const int64_t*, int, int64_t, int, int32_t*, double*,
+                  double*, int, cudaStream_t);
 
 }  // namespace lkb
 
@@ -402,7 +406,16 @@ int lkb_regress(const double* X, int x_batched, const double* y, const double* f
                 double* coeff_cov, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return regress(X, x_batched, y, flux_err, cadence_mask, prior_mu, prior_sigma, B, N, K, clip_sigma, niters, coeff,
-                 model, outlier_mask, status_out, coeff_cov, mem, (cudaStream_t)stream);
+                 model, outlier_mask, status_out, coeff_cov, mem, (cudaStream_t)stream, 0, 0);
+}
+
+int lkb_regress_ex(const double* X, int x_batched, const double* y, const double* flux_err,
+                   const uint8_t* cadence_mask, const double* prior_mu, const double* prior_sigma, int B, int64_t N,
+                   int K, double clip_sigma, int niters, double* coeff, double* model, uint8_t* outlier_mask,
+                   int32_t* status_out, double* coeff_cov, int mem, void* stream, int prior_batched, int flags) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return regress(X, x_batched, y, flux_err, cadence_mask, prior_mu, prior_sigma, B, N, K, clip_sigma, niters, coeff,
+                 model, outlier_mask, status_out, coeff_cov, mem, (cudaStream_t)stream, prior_batched, flags);
 }
 
 int lkb_elasticnet(const double* X, int x_batched, const double* y, const uint8_t* cadence_mask, int B, int64_t N,
@@ -411,6 +424,22 @@ int lkb_elasticnet(const double* X, int x_batched, const double* y, const uint8_
   std::lock_guard<std::mutex> lk(g_mu);
   return elasticnet(X, x_batched, y, cadence_mask, B, N, K, alpha, l1_ratio, max_iter, tol, positive, coeff, model,
                     n_iter, dual_gap, converged, mem, (cudaStream_t)stream);
+}
+
+int lkb_underfit_metric(const double* pool, int P, const double* target, int B, int64_t G, const int64_t* nb_offsets,
+                        const int32_t* nb_index, double* metric, int32_t* n_used, double* c3_mean, int mem,
+                        void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return underfit_metric(pool, P, target, B, G, nb_offsets, nb_index, metric, n_used, c3_mean, mem,
+                         (cudaStream_t)stream);
+}
+
+int lkb_overfit_terms(const float* corrected, const float* original, const float* noise, const int64_t* offsets, int B,
+                      int64_t F, int S, int32_t* n_positive, double* sum_positive, double* noise_mean, int mem,
+                      void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return overfit_terms(corrected, original, noise, offsets, B, F, S, n_positive, sum_positive, noise_mean, mem,
+                       (cudaStream_t)stream);
 }
 
 int lkb_savgol_tables(int window_length, int polyorder, double* coeffs, double* edge) {

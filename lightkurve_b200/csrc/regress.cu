@@ -310,8 +310,8 @@ rg_gram_mma_kernel(const double* __restrict__ X, int x_batched, const double* __
 // grad != NULL: iterative-refinement step - solve (A + prior) d = grad - prior (w - mu) for the current w = coeff and
 // write w + d (the matrix may be approximate, e.g. the tcgen05 Gram; grad is the exact fp64 gradient of the fit)
 __global__ void __launch_bounds__(256)
-rg_solve_kernel(int K, const double* __restrict__ prior_mu, const double* __restrict__ prior_sigma, RgWs ws,
-                double* __restrict__ coeff, int32_t* __restrict__ status, const double* __restrict__ grad,
+rg_solve_kernel(int K, const double* __restrict__ prior_mu, const double* __restrict__ prior_sigma, int64_t pstride,
+                RgWs ws, double* __restrict__ coeff, int32_t* __restrict__ status, const double* __restrict__ grad,
                 double* __restrict__ lu_out, int32_t* __restrict__ piv_out) {
   extern __shared__ __align__(16) double s_m[];        // [K][K+1] augmented
   __shared__ double s_red[8];
@@ -320,6 +320,7 @@ rg_solve_kernel(int K, const double* __restrict__ prior_mu, const double* __rest
   const int b = blockIdx.x;
   const int Ka = K + 1;
   const double* G = ws.gram + (int64_t)b * Ka * Ka;
+  if (prior_sigma) { prior_mu += pstride * b; prior_sigma += pstride * b; }   // pstride: 0 (shared [K]) or K ([B, K])
   // symmetric fill from the upper triangle (only blocks bi <= bj were accumulated, but inside a
   // diagonal block both triangles are present; use i <= j entries everywhere for exact symmetry)
   for (int e = threadIdx.x; e < K * Ka; e += blockDim.x) {
@@ -418,12 +419,13 @@ rg_solve_kernel(int K, const double* __restrict__ prior_mu, const double* __rest
 // d = (A + prior)^-1 [grad - prior (w - mu)], w <- w + d.  Two triangular solves instead of a second elimination
 // (the elimination is ~150 dependent block steps per light curve; the substitutions are one warp's dot products).
 __global__ void __launch_bounds__(256)
-rg_resolve_kernel(int K, const double* __restrict__ prior_mu, const double* __restrict__ prior_sigma,
+rg_resolve_kernel(int K, const double* __restrict__ prior_mu, const double* __restrict__ prior_sigma, int64_t pstride,
                   const double* __restrict__ lu, const int32_t* __restrict__ piv, double* __restrict__ coeff,
                   const int32_t* __restrict__ status, const double* __restrict__ grad) {
   extern __shared__ __align__(16) double s_m[];        // [K][K] factors, then the right-hand side [K]
   const int b = blockIdx.x;
   if (status && status[b] != LKB_OK) return;           // singular system: the coefficients are already NaN
+  if (prior_sigma) { prior_mu += pstride * b; prior_sigma += pstride * b; }
   double* s_r = s_m + (size_t)K * K;
   const double* LU = lu + (int64_t)b * K * K;
   for (int e = threadIdx.x; e < K * K; e += blockDim.x) s_m[e] = LU[e];
@@ -468,7 +470,7 @@ rg_resolve_kernel(int K, const double* __restrict__ prior_mu, const double* __re
 // ---- (A + prior)^-1 for propagate_errors (np.linalg.inv at regressioncorrector.py:185) -----------
 // Gauss-Jordan with partial pivoting on [M | I] held in an L2-resident global workspace [K][2K].
 __global__ void __launch_bounds__(256)
-rg_inverse_kernel(int K, const double* __restrict__ prior_sigma, RgWs ws, double* __restrict__ work,
+rg_inverse_kernel(int K, const double* __restrict__ prior_sigma, int64_t pstride, RgWs ws, double* __restrict__ work,
                   double* __restrict__ cov, const int32_t* __restrict__ status) {
   __shared__ double s_red[8];
   __shared__ int s_redi[8];
@@ -482,6 +484,7 @@ rg_inverse_kernel(int K, const double* __restrict__ prior_sigma, RgWs ws, double
     return;
   }
   const double* G = ws.gram + (int64_t)b * Ka * Ka;
+  if (prior_sigma) prior_sigma += pstride * b;
   double* M = work + (int64_t)b * K * W;
   for (int e = threadIdx.x; e < K * W; e += blockDim.x) {
     const int i = e / W, j = e % W;
@@ -624,10 +627,11 @@ __global__ void rg_zero_kernel(double* p, int64_t n, uint8_t* q, int64_t nq) {
 
 // The exact fp64 Gram pass over the listed rows: the FP64 tensor-core kernel when its tiling covers K + 1 columns,
 // else the SIMT kernel (LKB_REGRESS_SIMT=1 forces the SIMT kernel, kept for A/B measurements).  `sign` +1 adds the
-// rows, -1 removes them; `first` marks the first pass of a call (it may split a light curve over two CTAs).
+// rows, -1 removes them; `first` marks the first pass of a call (it may split a light curve over two CTAs).  With
+// `exact` the split depends on N alone, never on B, so a light curve's Gram matrix does not depend on the batch.
 // Shared by lkb_regress and lkb_elasticnet.
 static int rg_gram_pass(const double* d_X, int x_batched, const double* d_y, const double* d_fe, int B, int64_t N,
-                        int K, double sign, bool first, RgWs ws, cudaStream_t st) {
+                        int K, double sign, bool first, bool exact, RgWs ws, cudaStream_t st) {
   const int Ka = K + 1;
   const int ntile = (Ka + 7) / 8;
   const int tb = ntile <= 20 ? 4 : 5;
@@ -650,7 +654,7 @@ static int rg_gram_pass(const double* d_X, int x_batched, const double* d_y, con
   if (use_mma) {
     const size_t sm2 = 2 * sizeof(RgmStage);
     // first pass of a small batch: two CTAs per light curve to fill the SMs (wave quantisation)
-    const dim3 g((unsigned)B, (first && B < 4 * sm_count() && N >= 4096) ? 2u : 1u);
+    const dim3 g((unsigned)B, (first && (exact || B < 4 * sm_count()) && N >= 4096) ? 2u : 1u);
     const unsigned nt = 32u * nb5 * (nb5 + 1) / 2;
     if (tb == 5) rg_gram_mma_kernel<5, 5><<<g, nt, sm2, st>>>(d_X, x_batched, d_y, N, K, sign, ws);
     else switch (nb5) {
@@ -678,8 +682,12 @@ int regress_tc_gradient(const double* d_X, const double* d_y, const double* d_fe
 int regress(const double* X, int x_batched, const double* y, const double* flux_err, const uint8_t* cadence_mask,
             const double* prior_mu, const double* prior_sigma, int B, int64_t N, int K, double clip_sigma, int niters,
             double* coeff, double* model, uint8_t* outlier_mask, int32_t* status_out, double* coeff_cov, int mem,
-            cudaStream_t st) {
+            cudaStream_t st, int prior_batched, int flags) {
   LKB_REQUIRE(X && y && coeff && model && outlier_mask, "lkb_regress: null argument");
+  LKB_REQUIRE(prior_batched == 0 || prior_batched == 1, "lkb_regress_ex: prior_batched must be 0 or 1");
+  LKB_REQUIRE((flags & ~LKB_REGRESS_EXACT_INVARIANT) == 0, "lkb_regress_ex: unknown flags");
+  const bool exact = (flags & LKB_REGRESS_EXACT_INVARIANT) != 0;
+  const int64_t pstride = prior_batched ? K : 0;
   LKB_REQUIRE(B > 0 && B <= 65535 && N > 0 && K > 0 && niters >= 1, "lkb_regress: bad sizes");
   LKB_REQUIRE((prior_mu == nullptr) == (prior_sigma == nullptr), "Please specify both `prior_mu` and `prior_sigma`");
   LKB_REQUIRE(N < ((int64_t)1 << 31), "lkb_regress: N too large");
@@ -694,8 +702,8 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
   LKB_TRY(stage_in<double>(mem, WS_IN1, y, BN, &d_y, st));
   LKB_TRY(stage_in<double>(mem, WS_IN2, flux_err, BN, &d_fe, st));
   LKB_TRY(stage_in<uint8_t>(mem, WS_IN3, cadence_mask, BN, &d_cm, st));
-  LKB_TRY(stage_in<double>(mem, WS_IN4, prior_mu, K, &d_pm, st));
-  LKB_TRY(stage_in<double>(mem, WS_IN5, prior_sigma, K, &d_ps, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN4, prior_mu, (prior_batched ? (size_t)B : 1) * K, &d_pm, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN5, prior_sigma, (prior_batched ? (size_t)B : 1) * K, &d_ps, st));
 
   RgWs ws;
   LKB_TRY(ws_get_t<int32_t>(WS_A, BN, &ws.rows));
@@ -730,11 +738,13 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
     solve_attr = solve_smem;
   }
   // the first Gram pass of a large shared-design-matrix batch may take the tcgen05 GEMM; every other pass takes the
-  // exact fp64 kernels of rg_gram_pass (LKB_REGRESS_SIMT=1: SIMT kernels throughout, kept for A/B measurements)
+  // exact fp64 kernels of rg_gram_pass (LKB_REGRESS_SIMT=1: SIMT kernels throughout, kept for A/B measurements).
+  // LKB_REGRESS_EXACT_INVARIANT keeps every choice that depends on B or on a shared X out: no tcgen05 Gram, no batched
+  // model GEMM (the per-light-curve model of rg_clip / rg_final instead), the Gram split decided by N alone.
   static const bool force_simt = getenv("LKB_REGRESS_SIMT") != nullptr;
-  const bool use_tc = !force_simt && !x_batched && regress_tc_supported(B, N, K);
+  const bool use_tc = !exact && !force_simt && !x_batched && regress_tc_supported(B, N, K);
   // batched model X w as one FP64 tensor-core GEMM when the design matrix is shared by the batch
-  const bool gemm_model = !force_simt && !x_batched && K <= RGM_LD - 1 && B >= 8;
+  const bool gemm_model = !exact && !force_simt && !x_batched && K <= RGM_LD - 1 && B >= 8;
   dim3 gemm_grid(1, (unsigned)((B + RGE_LC - 1) / RGE_LC));
   if (gemm_model) {
     static bool attr = false;
@@ -762,7 +772,7 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
       // first fit of a large shared-design-matrix batch: the Gram matrices as one tcgen05 GEMM (regress_tc.cu)
       LKB_TRY(regress_tc_gram(d_X, d_y, d_fe, ws.used, B, N, K, ws.gram, st));
     } else {
-      LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, d_fe, B, N, K, it == 0 ? 1.0 : -1.0, it == 0, ws, st));
+      LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, d_fe, B, N, K, it == 0 ? 1.0 : -1.0, it == 0, exact, ws, st));
     }
     if (it == 0) { prof_end(st); prof_begin(st); }     // second record: everything after the first Gram pass
     LKB_LAUNCH_CHECK();
@@ -772,7 +782,7 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
       LKB_TRY(ws_get_t<double>(WS_Y0, (size_t)B * K * K, &d_lu));
       LKB_TRY(ws_get_t<int32_t>(WS_Y1, (size_t)B * K, &d_piv));
     }
-    rg_solve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, ws, o_c, d_status, nullptr, d_lu, d_piv);
+    rg_solve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, pstride, ws, o_c, d_status, nullptr, d_lu, d_piv);
     LKB_LAUNCH_CHECK();
     if (gemm_model) {
       rg_model_mma_kernel<<<gemm_grid, 256, sizeof(RgeSmem), st>>>(d_X, N, K, B, o_c, ws.resid);
@@ -787,9 +797,9 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
       LKB_TRY(ws_get_t<double>(WS_X6, (size_t)B * K, &d_grad));
       LKB_TRY(regress_tc_gradient(d_X, d_y, d_fe, ws.used, ws.resid, B, N, K, d_grad, st));
       if (getenv("LKB_REGRESS_REFACTOR"))            // (A/B: eliminate again instead of reusing the factors)
-        rg_solve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, ws, o_c, d_status, d_grad, nullptr, nullptr);
+        rg_solve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, pstride, ws, o_c, d_status, d_grad, nullptr, nullptr);
       else
-        rg_resolve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, d_lu, d_piv, o_c, d_status, d_grad);
+        rg_resolve_kernel<<<B, 256, solve_smem, st>>>(K, d_pm, d_ps, pstride, d_lu, d_piv, o_c, d_status, d_grad);
       LKB_LAUNCH_CHECK();
       rg_model_mma_kernel<<<gemm_grid, 256, sizeof(RgeSmem), st>>>(d_X, N, K, B, o_c, ws.resid);
       LKB_LAUNCH_CHECK();
@@ -808,7 +818,7 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
     // but the ones found by the final clip, exactly like the reference's last _fit_coefficients call)
     double* d_work = nullptr;
     LKB_TRY(ws_get_t<double>(WS_F, (size_t)B * K * 2 * K, &d_work));
-    rg_inverse_kernel<<<B, 256, 0, st>>>(K, d_ps, ws, d_work, o_cov, d_status);
+    rg_inverse_kernel<<<B, 256, 0, st>>>(K, d_ps, pstride, ws, d_work, o_cov, d_status);
     LKB_LAUNCH_CHECK();
   }
 
@@ -894,7 +904,7 @@ int elasticnet(const double* X, int x_batched, const double* y, const uint8_t* c
     }
   }
   prof_begin(st);
-  LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, nullptr, B, N, K, 1.0, true, ws, st));
+  LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, nullptr, B, N, K, 1.0, true, false, ws, st));
   LKB_LAUNCH_CHECK();
   prof_end(st);
   prof_begin(st);

@@ -430,10 +430,15 @@ def flatten(times, fluxes, flux_errs=None, masks=None, window_length=101, polyor
 # regression
 # --------------------------------------------------------------------------------------
 def regress(X, Y, flux_err=None, cadence_mask=None, prior_mu=None, prior_sigma=None, sigma=5, niters=5,
-            return_cov=False):
+            return_cov=False, exact_invariant=False):
     """K5.  X [N, K] (shared) or [B, N, K]; Y [B, N]; flux_err [B, N] or None (ones);
-    cadence_mask bool [B, N] or None.  Returns dict(coefficients [B,K], model [B,N]
-    (median-subtracted), outlier_mask bool [B,N], status int32 [B])."""
+    cadence_mask bool [B, N] or None; prior_mu / prior_sigma [K] (shared) or [B, K] (one prior per light curve).
+    `exact_invariant`: each light curve's results are bitwise independent of the batch and of a shared or batched X
+    (LKB_REGRESS_EXACT_INVARIANT).  Returns dict(coefficients [B,K], model [B,N] (median-subtracted), outlier_mask
+    bool [B,N], status int32 [B]).  With CUDA torch tensors (float64; cadence_mask uint8) the call runs in device
+    mode on the current stream and returns tensors (outlier_mask uint8)."""
+    if _is_torch(Y):
+        return _regress_device(X, Y, flux_err, cadence_mask, prior_mu, prior_sigma, sigma, niters, exact_invariant)
     lib = L.load()
     X = np.ascontiguousarray(X, dtype=np.float64)
     Y = np.ascontiguousarray(np.atleast_2d(Y), dtype=np.float64)
@@ -447,18 +452,59 @@ def regress(X, Y, flux_err=None, cadence_mask=None, prior_mu=None, prior_sigma=N
         np.ascontiguousarray(np.broadcast_to(np.asarray(cadence_mask, dtype=bool), Y.shape).astype(np.uint8))
     pm = None if prior_mu is None else np.ascontiguousarray(prior_mu, dtype=np.float64)
     ps = None if prior_sigma is None else np.ascontiguousarray(prior_sigma, dtype=np.float64)
+    prior_batched = ps is not None and ps.ndim == 2
+    for name, v in (("prior_mu", pm), ("prior_sigma", ps)):
+        if v is not None and v.shape != ((B, K) if prior_batched else (K,)):
+            raise ValueError("%s must have shape (%d,) or (%d, %d), got %s" % (name, K, B, K, v.shape))
     coeff = np.empty((B, K), dtype=np.float64)
     model = np.empty((B, N), dtype=np.float64)
     om = np.empty((B, N), dtype=np.uint8)
     status = np.empty(B, dtype=np.int32)
     cov = np.empty((B, K, K), dtype=np.float64) if return_cov else None
-    L.check(lib.lkb_regress(L.ptr(X), 1 if batched else 0, L.ptr(Y), L.ptr(fe), L.ptr(cm), L.ptr(pm), L.ptr(ps),
-                            B, N, K, float(sigma), int(niters), L.ptr(coeff), L.ptr(model), L.ptr(om),
-                            L.ptr(status), L.ptr(cov), L.MEM_HOST, None))
+    L.check(lib.lkb_regress_ex(L.ptr(X), 1 if batched else 0, L.ptr(Y), L.ptr(fe), L.ptr(cm), L.ptr(pm), L.ptr(ps),
+                               B, N, K, float(sigma), int(niters), L.ptr(coeff), L.ptr(model), L.ptr(om),
+                               L.ptr(status), L.ptr(cov), L.MEM_HOST, None, 1 if prior_batched else 0,
+                               L.REGRESS_EXACT_INVARIANT if exact_invariant else 0))
     out = dict(coefficients=coeff, model=model, outlier_mask=om.astype(bool), status=status)
     if return_cov:
         out["covariance"] = cov
     return out
+
+
+def _regress_device(X, Y, flux_err, cadence_mask, prior_mu, prior_sigma, sigma, niters, exact_invariant):
+    import torch
+    lib = L.load()
+    for name, t, dt in (("X", X, torch.float64), ("Y", Y, torch.float64), ("flux_err", flux_err, torch.float64),
+                        ("cadence_mask", cadence_mask, torch.uint8), ("prior_mu", prior_mu, torch.float64),
+                        ("prior_sigma", prior_sigma, torch.float64)):
+        if t is not None and not (_is_torch(t) and t.is_cuda and t.is_contiguous() and t.dtype == dt):
+            raise ValueError("%s must be a contiguous CUDA %s tensor in device mode" % (name, dt))
+    if Y.dim() != 2:
+        raise ValueError("Y must be [B, N]")
+    B, N = Y.shape
+    batched = X.dim() == 3
+    K = X.shape[-1]
+    if X.shape[-2] != N or (batched and X.shape[0] != B):
+        raise ValueError("X shape %s does not match Y shape %s" % (tuple(X.shape), tuple(Y.shape)))
+    for name, t in (("flux_err", flux_err), ("cadence_mask", cadence_mask)):
+        if t is not None and tuple(t.shape) != (B, N):
+            raise ValueError("%s must be [B, N]" % name)
+    if (prior_mu is None) != (prior_sigma is None):
+        raise ValueError("Please specify both `prior_mu` and `prior_sigma`")
+    prior_batched = prior_sigma is not None and prior_sigma.dim() == 2
+    for name, v in (("prior_mu", prior_mu), ("prior_sigma", prior_sigma)):
+        if v is not None and tuple(v.shape) != ((B, K) if prior_batched else (K,)):
+            raise ValueError("%s must have shape (%d,) or (%d, %d)" % (name, K, B, K))
+    dev = Y.device
+    coeff = torch.empty((B, K), dtype=torch.float64, device=dev)
+    model = torch.empty((B, N), dtype=torch.float64, device=dev)
+    om = torch.empty((B, N), dtype=torch.uint8, device=dev)
+    status = torch.empty(B, dtype=torch.int32, device=dev)
+    L.check(lib.lkb_regress_ex(L.ptr(X), 1 if batched else 0, L.ptr(Y), L.ptr(flux_err), L.ptr(cadence_mask),
+                               L.ptr(prior_mu), L.ptr(prior_sigma), B, N, K, float(sigma), int(niters), L.ptr(coeff),
+                               L.ptr(model), L.ptr(om), L.ptr(status), None, L.MEM_DEVICE, _stream_ptr(),
+                               1 if prior_batched else 0, L.REGRESS_EXACT_INVARIANT if exact_invariant else 0))
+    return dict(coefficients=coeff, model=model, outlier_mask=om, status=status)
 
 
 def elasticnet(X, Y, cadence_mask=None, alpha=1e-20, l1_ratio=0.01, max_iter=1000, tol=1e-4, positive=False):
@@ -485,6 +531,92 @@ def elasticnet(X, Y, cadence_mask=None, alpha=1e-20, l1_ratio=0.01, max_iter=100
                                float(l1_ratio), int(max_iter), float(tol), 1 if positive else 0, L.ptr(coeff),
                                L.ptr(model), L.ptr(n_iter), L.ptr(gap), L.ptr(conv), L.MEM_HOST, None))
     return dict(coefficients=coeff, model=model, n_iter=n_iter, dual_gap=gap, converged=conv.astype(bool))
+
+
+def _k9_array(x, dtype, torch_dtype_name):
+    """(array or tensor, mem) for a K9 input: CUDA torch tensors are passed through (device mode)."""
+    if _is_torch(x):
+        if not (x.is_cuda and x.is_contiguous() and str(x.dtype) == "torch." + torch_dtype_name):
+            raise ValueError("device inputs must be contiguous CUDA %s tensors" % torch_dtype_name)
+        return x, L.MEM_DEVICE
+    return np.ascontiguousarray(x, dtype=dtype), L.MEM_HOST
+
+
+def underfit_metric(pool, target, nb_offsets, nb_index):
+    """K9.  The under-fitting metric of metrics.py:178-255 for B targets whose neighbours are rows of one pool.
+    pool [P, G] and target [B, G] fp64 on one cadence grid, NaN where a value is absent (numpy, or CUDA torch tensors
+    for device mode); nb_offsets int64 [B + 1] and nb_index [nb_offsets[-1]] (host): the pool rows of each target.
+    Returns dict(metric [B], n_used int32 [B] (cadences used), c3_mean [B] (the nanmean of |c|^3)), numpy or torch."""
+    lib = L.load()
+    pool, mem = _k9_array(pool, np.float64, "float64")
+    target, mem_t = _k9_array(target, np.float64, "float64")
+    if mem != mem_t:
+        raise ValueError("pool and target must both be host arrays or both CUDA tensors")
+    if pool.ndim != 2 or target.ndim != 2 or pool.shape[1] != target.shape[1]:
+        raise ValueError("pool [P, G] and target [B, G] must share G")
+    P, G = pool.shape
+    B = target.shape[0]
+    off = np.ascontiguousarray(nb_offsets, dtype=np.int64)
+    idx = np.ascontiguousarray(nb_index, dtype=np.int32)
+    if off.shape != (B + 1,) or len(idx) != off[-1]:
+        raise ValueError("nb_offsets must have B + 1 entries and end at len(nb_index)")
+    if mem == L.MEM_DEVICE:
+        import torch
+        metric = torch.empty(B, dtype=torch.float64, device=target.device)
+        n_used = torch.empty(B, dtype=torch.int32, device=target.device)
+        c3 = torch.empty(B, dtype=torch.float64, device=target.device)
+        stream = _stream_ptr()
+    else:
+        metric, n_used, c3, stream = np.empty(B), np.empty(B, np.int32), np.empty(B), None
+    L.check(lib.lkb_underfit_metric(L.ptr(pool), P, L.ptr(target), B, G, L.ptr(off), L.ptr(idx), L.ptr(metric),
+                                    L.ptr(n_used), L.ptr(c3), mem, stream))
+    return dict(metric=metric, n_used=n_used, c3_mean=c3)
+
+
+def overfit_terms(corrected, original, noise, offsets=None, n_samples=1):
+    """K9.  The per-light-curve terms of the over-fitting metric (metrics.py:23-123) from float32 power rows.
+    corrected / original: [B, F] (one grid) or the rows back to back with `offsets` int64 [B + 1] (host); noise: the
+    `n_samples` noise rows of each light curve back to back (light curve b's rows at n_samples * offsets[b]).  numpy,
+    or CUDA torch tensors for device mode.  Returns dict(n_positive int32 [B], sum_positive [B],
+    noise_mean [B, n_samples])."""
+    lib = L.load()
+    corrected, mem = _k9_array(corrected, np.float32, "float32")
+    original, _ = _k9_array(original, np.float32, "float32")
+    S = int(n_samples)
+    if offsets is None:
+        if corrected.ndim != 2:
+            raise ValueError("without offsets the power rows must be [B, F]")
+        B, F = corrected.shape
+        off = None
+    else:
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        if off.ndim != 1 or len(off) < 2 or off[0] != 0 or np.any(np.diff(off) < 0):
+            raise ValueError("offsets must be an ascending int64 CSR array starting at 0")
+        B, F = len(off) - 1, 0
+    if tuple(original.shape) != tuple(corrected.shape):
+        raise ValueError("corrected and original power must have the same shape")
+    n_tot = B * F if off is None else int(off[-1])
+    n_rows = corrected.numel() if mem == L.MEM_DEVICE else corrected.size
+    if n_rows != n_tot:
+        raise ValueError("offsets end at %d but the power rows hold %d values" % (n_tot, n_rows))
+    if S > 0:
+        noise, _ = _k9_array(noise, np.float32, "float32")
+        if (noise.numel() if mem == L.MEM_DEVICE else noise.size) != S * n_tot:
+            raise ValueError("noise must hold n_samples rows per light curve")
+    else:
+        noise = None
+    if mem == L.MEM_DEVICE:
+        import torch
+        dev = corrected.device
+        npos = torch.empty(B, dtype=torch.int32, device=dev)
+        spos = torch.empty(B, dtype=torch.float64, device=dev)
+        nmean = torch.empty((B, S), dtype=torch.float64, device=dev)
+        stream = _stream_ptr()
+    else:
+        npos, spos, nmean, stream = np.empty(B, np.int32), np.empty(B), np.empty((B, S)), None
+    L.check(lib.lkb_overfit_terms(L.ptr(corrected), L.ptr(original), L.ptr(noise), L.ptr(off), B, F, S, L.ptr(npos),
+                                  L.ptr(spos), L.ptr(nmean) if S else None, mem, stream))
+    return dict(n_positive=npos, sum_positive=spos, noise_mean=nmean)
 
 
 def nanmedian_std(arrays):
