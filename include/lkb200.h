@@ -178,6 +178,49 @@ int lkb_bls_power_ex(const double* t, const double* y, const double* dy, const i
                      double* transit_time, double* depth_snr, double* log_likelihood,
                      int32_t* best_bins, int mem, void* stream);
 
+/* K10: the vetting step after the search, one candidate (period, duration, transit_time) per light curve -
+ * BoxLeastSquaresPeriodogram.compute_stats (periodogram.py:1194-1229) and the mask of get_transit_mask
+ * (periodogram.py:1275-1296) for B light curves in one call.
+ *   t, y, dy        [offsets[B]] fp64, raw times and fluxes (dy NULL: unit weights); times in any order; every light
+ *                   curve has at least one cadence
+ *   offsets         HOST CSR [B+1]
+ *   period, duration, transit_time  [B] fp64 (transit_time absolute, in the units of t); period and duration > 0
+ *   transit_offsets HOST CSR [B+1]: the per-transit slots of light curve b are transit_offsets[b] ..
+ *                   transit_offsets[b+1]-1.  With tt = transit_time - t[first cadence], a light curve needs at most
+ *                     rint((max t - t[0] - tt) / P) - rint((min t - t[0] - tt) / P) + 1
+ *                   slots (times measured from its first cadence, as compute_stats does).
+ *   stats           [B, LKB_BLS_STATS_NCOL] out, columns below
+ *   transit_first   [B] int64 out: id rint((t - t[0] - tt) / P) of the first transit with an in-transit cadence (0 if none)
+ *   transit_n       [B] int32 out: transit ids used, last - first + 1 (0 if no cadence is in transit)
+ *   per_transit_count, per_transit_ll  [transit_offsets[B]] out: cadences and log-likelihood of each transit, first
+ *                   id first (compute_stats' per_transit_count / per_transit_log_likelihood); a light curve's
+ *                   slots past its transit_n[b] are 0
+ *   in_transit      [offsets[B]] uint8 out or NULL: 1 where the box model of get_transit_model is in transit
+ *   status          [B] int32 out: LKB_OK; LKB_E_SINGULAR when the sine fit's normal equations have an exactly zero
+ *                   pivot (numpy's LinAlgError: harmonic columns NaN, everything else valid); LKB_E_ARG when the light
+ *                   curve needs more transit slots than it was given (its per-transit slots are left 0)
+ * Returns LKB_E_ARG for a non-positive or non-finite period / duration, a non-finite transit_time, an empty light
+ * curve, or when any light curve lacks transit slots (never truncated).  The masks, transit ids and counts are
+ * bit-exact; each light curve's results are bitwise independent of the rest of the batch and of the run.  Host mode
+ * is synchronous; device mode enqueues the kernel on `stream` but, like host mode, reads period / duration /
+ * transit_time first and synchronises once at the end to check the slot capacities. */
+#define LKB_BLS_STATS_NCOL               15
+#define LKB_BLS_STATS_DEPTH               0   /* (depth, depth_err): in-transit vs out-of-transit */
+#define LKB_BLS_STATS_DEPTH_ODD           2   /* (depth, err) of the odd transits */
+#define LKB_BLS_STATS_DEPTH_EVEN          4   /* (depth, err) of the even transits */
+#define LKB_BLS_STATS_DEPTH_HALF          6   /* (depth, err) at half the period */
+#define LKB_BLS_STATS_DEPTH_PHASED        8   /* (depth, err) half a period after the transit */
+#define LKB_BLS_STATS_HARMONIC_AMPLITUDE 10   /* amplitude of the best sine fit at the period */
+#define LKB_BLS_STATS_HARMONIC_DELTA_LOGLIKE 11  /* log-likelihood of the sine fit minus that of the box */
+#define LKB_BLS_STATS_Y_IN               12   /* get_transit_model's in-transit level (NaN without in-transit cadences) */
+#define LKB_BLS_STATS_Y_OUT              13   /* its out-of-transit level (NaN when every cadence is in transit) */
+#define LKB_BLS_STATS_N_IN               14   /* its in-transit cadences (= the ones of in_transit) */
+int lkb_bls_stats(const double* t, const double* y, const double* dy, const int64_t* offsets, int B,
+                  const double* period, const double* duration, const double* transit_time,
+                  const int64_t* transit_offsets, double* stats, int64_t* transit_first, int32_t* transit_n,
+                  int32_t* per_transit_count, double* per_transit_ll, uint8_t* in_transit, int32_t* status,
+                  int mem, void* stream);
+
 /* Debug/parity entry: the per-sample bin index of bls.c for ONE period,
  * ind[n] = (int)(fabs(fmod(t[n]-min_t, period))/bin_duration)+1, evaluated by the
  * same device function the search kernel uses. */

@@ -216,6 +216,9 @@ int bls_power(const double*, const double*, const double*, const int64_t*, int, 
               int64_t, const double*, int, int, int, double*, double*, double*, double*, double*, double*, double*,
               int32_t*, int, cudaStream_t);
 int bls_bin_index(const double*, int64_t, double, double, double, int32_t*, int, cudaStream_t);
+int bls_stats(const double*, const double*, const double*, const int64_t*, int, const double*, const double*,
+              const double*, const int64_t*, double*, int64_t*, int32_t*, int32_t*, double*, uint8_t*, int32_t*, int,
+              cudaStream_t);
 int flatten(const double*, const double*, const double*, const uint8_t*, const int64_t*, int, int, int, double, int,
             double, double*, double*, double*, int, cudaStream_t);
 int regress(const double*, int, const double*, const double*, const uint8_t*, const double*, const double*, int,
@@ -388,6 +391,16 @@ int lkb_bls_bin_index(const double* t_rel, int64_t N, double min_t, double perio
                       int32_t* ind, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return bls_bin_index(t_rel, N, min_t, period, bin_duration, ind, mem, (cudaStream_t)stream);
+}
+
+int lkb_bls_stats(const double* t, const double* y, const double* dy, const int64_t* offsets, int B,
+                  const double* period, const double* duration, const double* transit_time,
+                  const int64_t* transit_offsets, double* stats, int64_t* transit_first, int32_t* transit_n,
+                  int32_t* per_transit_count, double* per_transit_ll, uint8_t* in_transit, int32_t* status, int mem,
+                  void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return bls_stats(t, y, dy, offsets, B, period, duration, transit_time, transit_offsets, stats, transit_first,
+                   transit_n, per_transit_count, per_transit_ll, in_transit, status, mem, (cudaStream_t)stream);
 }
 
 int lkb_flatten(const double* time, const double* flux, const double* flux_err, const uint8_t* exclude_mask,

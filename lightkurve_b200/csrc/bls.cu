@@ -28,22 +28,12 @@
 #include "common.cuh"
 #include "select.cuh"
 #include "bls_plan.h"
+#include "bls_stats.cuh"     // K10 (vetting statistics), and bls_fmod
 #include <float.h>
 #include <algorithm>
 #include <vector>
 
 namespace lkb {
-
-// exact fmod for finite x, p != 0, |x/p| < 2^50 (true for any real light curve)
-__device__ __forceinline__ double bls_fmod(double x, double p, double inv_p) {
-  const double a = fabs(x), b = fabs(p);
-  if (a < b) return x;
-  double q = trunc(a * inv_p);
-  double r = fma(-q, b, a);
-  if (r < 0.0) { q -= 1.0; r = fma(-q, b, a); }
-  else if (r >= b) { q += 1.0; r = fma(-q, b, a); }
-  return copysign(r, x);
-}
 
 // (int)(r / bd) with the IEEE division replaced, on the fast path, by a reciprocal multiply whose
 // result is PROVEN equal: k = trunc(r * (1/bd)); rem = fma(-k, bd, r) is the (once rounded) remainder;
@@ -764,6 +754,104 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
   LKB_TRY(stage_out_copy<double>(mem, log_like, o6, outn, st));
   LKB_TRY(stage_out_copy<int32_t>(mem, best_bins, ob, 2 * outn, st));
   if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+  return LKB_OK;
+}
+
+int bls_stats(const double* t, const double* y, const double* dy, const int64_t* h_offsets, int B,
+              const double* period, const double* duration, const double* transit_time, const int64_t* h_toff,
+              double* stats, int64_t* transit_first, int32_t* transit_n, int32_t* per_transit_count,
+              double* per_transit_ll, uint8_t* in_transit, int32_t* status, int mem, cudaStream_t st) {
+  LKB_REQUIRE(t && y && h_offsets && period && duration && transit_time && h_toff, "lkb_bls_stats: null input");
+  LKB_REQUIRE(stats && transit_first && transit_n && status, "lkb_bls_stats: null output");
+  LKB_REQUIRE(B > 0, "lkb_bls_stats: B must be > 0");
+  LKB_REQUIRE(h_offsets[0] == 0 && h_toff[0] == 0, "lkb_bls_stats: offsets[0] and transit_offsets[0] must be 0");
+  for (int b = 0; b < B; ++b) {
+    const int64_t nb = h_offsets[b + 1] - h_offsets[b];
+    if (nb < 1 || nb >= ((int64_t)1 << 31)) {
+      set_error("lkb_bls_stats: light curve %d has %lld cadences (1 .. 2^31 - 1 supported)", b, (long long)nb);
+      return LKB_E_ARG;
+    }
+    if (h_toff[b + 1] < h_toff[b]) {
+      set_error("lkb_bls_stats: transit_offsets decrease at light curve %d", b);
+      return LKB_E_ARG;
+    }
+  }
+  const int64_t total = h_offsets[B], slots = h_toff[B];
+  LKB_REQUIRE(slots == 0 || (per_transit_count && per_transit_ll), "lkb_bls_stats: null per-transit output");
+  LKB_TRY(ensure_device());
+
+  // the candidates are checked on the host
+  std::vector<double> h_cand(3 * (size_t)B);
+  const double* cand[3] = {period, duration, transit_time};
+  for (int k = 0; k < 3; ++k) {
+    if (mem == LKB_MEM_HOST) memcpy(h_cand.data() + (size_t)k * B, cand[k], sizeof(double) * B);
+    else LKB_CUDA_CHECK(cudaMemcpyAsync(h_cand.data() + (size_t)k * B, cand[k], sizeof(double) * B,
+                                        cudaMemcpyDeviceToHost, st));
+  }
+  if (mem != LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    const double p = h_cand[b], d = h_cand[(size_t)B + b], tt = h_cand[2 * (size_t)B + b];
+    if (!(p > 0.0) || isinf(p) || !(d > 0.0) || isinf(d)) {
+      set_error("lkb_bls_stats: light curve %d: period (%g) and duration (%g) must be positive and finite", b, p, d);
+      return LKB_E_ARG;
+    }
+    if (!isfinite(tt)) {
+      set_error("lkb_bls_stats: light curve %d: transit_time is not finite", b);
+      return LKB_E_ARG;
+    }
+  }
+
+  const double *d_t = nullptr, *d_y = nullptr, *d_dy = nullptr, *d_p = nullptr, *d_d = nullptr, *d_tt = nullptr;
+  LKB_TRY(stage_in<double>(mem, WS_IN0, t, total, &d_t, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN1, y, total, &d_y, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN2, dy, total, &d_dy, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN3, period, B, &d_p, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN4, duration, B, &d_d, st));
+  LKB_TRY(stage_in<double>(mem, WS_IN5, transit_time, B, &d_tt, st));
+  int64_t *d_off = nullptr, *d_toff = nullptr;
+  LKB_TRY(ws_get_t<int64_t>(WS_A, (size_t)B + 1, &d_off));
+  LKB_TRY(ws_get_t<int64_t>(WS_B, (size_t)B + 1, &d_toff));
+  LKB_CUDA_CHECK(cudaMemcpyAsync(d_off, h_offsets, sizeof(int64_t) * (B + 1), cudaMemcpyHostToDevice, st));
+  LKB_CUDA_CHECK(cudaMemcpyAsync(d_toff, h_toff, sizeof(int64_t) * (B + 1), cudaMemcpyHostToDevice, st));
+  double *o_st = nullptr, *o_ll = nullptr;
+  int64_t* o_first = nullptr;
+  int32_t *o_n = nullptr, *o_cnt = nullptr, *o_status = nullptr;
+  uint8_t* o_mask = nullptr;
+  LKB_TRY(stage_out_alloc<double>(mem, WS_OUT0, stats, (size_t)B * LKB_BLS_STATS_NCOL, &o_st));
+  LKB_TRY(stage_out_alloc<int64_t>(mem, WS_OUT1, transit_first, B, &o_first));
+  LKB_TRY(stage_out_alloc<int32_t>(mem, WS_OUT2, transit_n, B, &o_n));
+  LKB_TRY(stage_out_alloc<int32_t>(mem, WS_OUT3, slots ? per_transit_count : nullptr, slots, &o_cnt));
+  LKB_TRY(stage_out_alloc<double>(mem, WS_OUT4, slots ? per_transit_ll : nullptr, slots, &o_ll));
+  LKB_TRY(stage_out_alloc<uint8_t>(mem, WS_OUT5, in_transit, total, &o_mask));
+  LKB_TRY(stage_out_alloc<int32_t>(mem, WS_OUT6, status, B, &o_status));
+  prof_begin(st);
+  LKB_TRY(bls_stats_launch(d_t, d_y, d_dy, d_off, B, d_p, d_d, d_tt, d_toff, o_st, o_first, o_n, o_cnt, o_ll, o_mask,
+                           o_status, st));
+  prof_end(st);
+  LKB_TRY(stage_out_copy<double>(mem, stats, o_st, (size_t)B * LKB_BLS_STATS_NCOL, st));
+  LKB_TRY(stage_out_copy<int64_t>(mem, transit_first, o_first, B, st));
+  LKB_TRY(stage_out_copy<int32_t>(mem, transit_n, o_n, B, st));
+  LKB_TRY(stage_out_copy<int32_t>(mem, slots ? per_transit_count : nullptr, o_cnt, slots, st));
+  LKB_TRY(stage_out_copy<double>(mem, slots ? per_transit_ll : nullptr, o_ll, slots, st));
+  LKB_TRY(stage_out_copy<uint8_t>(mem, in_transit, o_mask, total, st));
+  LKB_TRY(stage_out_copy<int32_t>(mem, status, o_status, B, st));
+  // slot capacity: read the statuses (and the slots each light curve needed) back
+  std::vector<int32_t> h_status(B), h_n(B);
+  if (mem == LKB_MEM_HOST) {
+    LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+    memcpy(h_status.data(), status, sizeof(int32_t) * B);
+    memcpy(h_n.data(), transit_n, sizeof(int32_t) * B);
+  } else {
+    LKB_CUDA_CHECK(cudaMemcpyAsync(h_status.data(), status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+    LKB_CUDA_CHECK(cudaMemcpyAsync(h_n.data(), transit_n, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+    LKB_CUDA_CHECK(cudaStreamSynchronize(st));
+  }
+  for (int b = 0; b < B; ++b)
+    if (h_status[b] == LKB_E_ARG) {
+      set_error("lkb_bls_stats: light curve %d needs %d transit slots, transit_offsets gives it %lld", b, h_n[b],
+                (long long)(h_toff[b + 1] - h_toff[b]));
+      return LKB_E_ARG;
+    }
   return LKB_OK;
 }
 

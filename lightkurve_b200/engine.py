@@ -358,6 +358,111 @@ def bls_power(times, fluxes, flux_errs, period, duration, oversample=10, objecti
     return res
 
 
+BLS_STATS_COLUMNS = ("depth", "depth_err", "depth_odd", "depth_odd_err", "depth_even", "depth_even_err", "depth_half",
+                     "depth_half_err", "depth_phased", "depth_phased_err", "harmonic_amplitude",
+                     "harmonic_delta_log_likelihood", "y_in", "y_out", "n_in")     # LKB_BLS_STATS_* in lkb200.h
+
+
+def bls_transit_slots(times, period, transit_time):
+    """Per-transit slot capacity of each light curve as a HOST CSR int64 [B + 1] (the bound of lkb200.h): with times
+    and tt = transit_time - t[0] measured from the first cadence, rint((max t - tt) / P) - rint((min t - tt) / P) + 1."""
+    caps = np.zeros(len(times) + 1, dtype=np.int64)
+    for b, (t, p, tt) in enumerate(zip(times, period, transit_time)):
+        t = np.asarray(t, dtype=np.float64)
+        t0 = t[0]
+        ttr = float(tt) - t0
+        lo = np.rint((t.min() - t0 - ttr) / float(p))
+        hi = np.rint((t.max() - t0 - ttr) / float(p))
+        caps[b + 1] = int(hi - lo) + 1
+    return np.cumsum(caps)
+
+
+def bls_stats(times, fluxes, flux_errs, period, duration, transit_time, return_mask=False, offsets=None,
+              transit_offsets=None):
+    """K10.  The vetting statistics of BoxLeastSquaresPeriodogram.compute_stats and the mask of get_transit_mask for one
+    candidate per light curve.  `period`, `duration`, `transit_time` (absolute): [B] or scalars.
+    Host mode: lists of per-light-curve arrays (flux_errs: list or None => unit weights); the slot capacity is
+    computed here (bls_transit_slots).  Device mode: `times`, `fluxes` (and `flux_errs` or None) are the concatenated
+    CUDA float64 tensors with `offsets` (host int64 [B + 1]), the candidates CUDA float64 tensors [B], and
+    `transit_offsets` (host int64 [B + 1]) is required.
+    Returns dict(stats [B, len(BLS_STATS_COLUMNS)], transit_first int64 [B], transit_n int32 [B],
+    per_transit_count int32 and per_transit_log_likelihood [transit_offsets[-1]] (light curve b's transits at
+    transit_offsets[b], transit_n[b] of them), status int32 [B] (0 or -4 = singular sine fit), offsets,
+    transit_offsets and, with return_mask, in_transit (bool on the host, uint8 on the device) [offsets[-1]])."""
+    lib = L.load()
+    if _is_torch(times):
+        return _bls_stats_device(lib, times, fluxes, flux_errs, period, duration, transit_time, return_mask, offsets,
+                                 transit_offsets)
+    B = len(times)
+    t, offsets = _csr(times)
+    y, yoff = _csr(fluxes)
+    if not np.array_equal(offsets, yoff):
+        raise ValueError("time and flux lengths differ")
+    dy = None
+    if flux_errs is not None:
+        dy, doff = _csr(flux_errs)
+        if not np.array_equal(offsets, doff):
+            raise ValueError("time and flux_err lengths differ")
+    cand = [np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (B,))) for x in
+            (period, duration, transit_time)]
+    if np.any(np.diff(offsets) < 1):
+        raise ValueError("light curve %d has no cadences" % int(np.flatnonzero(np.diff(offsets) < 1)[0]))
+    bad = ~((cand[0] > 0) & np.isfinite(cand[0]) & (cand[1] > 0) & np.isfinite(cand[1]) & np.isfinite(cand[2]))
+    if np.any(bad):
+        b = int(np.flatnonzero(bad)[0])
+        raise ValueError("light curve %d: period (%g) and duration (%g) must be positive and finite, transit_time (%g) "
+                         "finite" % (b, cand[0][b], cand[1][b], cand[2][b]))
+    if transit_offsets is None:
+        transit_offsets = bls_transit_slots(times, cand[0], cand[2])
+    toff = np.ascontiguousarray(transit_offsets, dtype=np.int64)
+    slots = int(toff[-1])
+    stats = np.empty((B, len(BLS_STATS_COLUMNS)))
+    first, n_tr, status = np.empty(B, np.int64), np.empty(B, np.int32), np.empty(B, np.int32)
+    cnt, ll = np.empty(slots, np.int32), np.empty(slots)
+    mask = np.empty(len(t), np.uint8) if return_mask else None
+    L.check(lib.lkb_bls_stats(L.ptr(t), L.ptr(y), L.ptr(dy), L.ptr(offsets), B, *[L.ptr(c) for c in cand], L.ptr(toff),
+                              L.ptr(stats), L.ptr(first), L.ptr(n_tr), L.ptr(cnt) if slots else None,
+                              L.ptr(ll) if slots else None, L.ptr(mask), L.ptr(status), L.MEM_HOST, None))
+    res = dict(stats=stats, transit_first=first, transit_n=n_tr, per_transit_count=cnt, per_transit_log_likelihood=ll,
+               status=status, offsets=offsets, transit_offsets=toff)
+    if return_mask:
+        res["in_transit"] = mask.view(bool)
+    return res
+
+
+def _bls_stats_device(lib, t, y, dy, period, duration, transit_time, return_mask, offsets, transit_offsets):
+    import torch
+    if offsets is None or transit_offsets is None:
+        raise ValueError("device mode needs the host CSR `offsets` and `transit_offsets`")
+    for name, x in (("times", t), ("fluxes", y), ("flux_errs", dy), ("period", period), ("duration", duration),
+                    ("transit_time", transit_time)):
+        if x is not None and not (_is_torch(x) and x.is_cuda and x.is_contiguous() and x.dtype == torch.float64):
+            raise ValueError("device mode: %s must be a contiguous CUDA float64 tensor" % name)
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    toff = np.ascontiguousarray(transit_offsets, dtype=np.int64)
+    B = len(off) - 1
+    if t.numel() != off[-1] or y.numel() != off[-1] or (dy is not None and dy.numel() != off[-1]):
+        raise ValueError("offsets end at %d but the arrays hold %d values" % (off[-1], t.numel()))
+    if period.numel() != B or duration.numel() != B or transit_time.numel() != B:
+        raise ValueError("period, duration and transit_time need one value per light curve")
+    dev, slots = t.device, int(toff[-1])
+    stats = torch.empty((B, len(BLS_STATS_COLUMNS)), dtype=torch.float64, device=dev)
+    first = torch.empty(B, dtype=torch.int64, device=dev)
+    n_tr = torch.empty(B, dtype=torch.int32, device=dev)
+    status = torch.empty(B, dtype=torch.int32, device=dev)
+    cnt = torch.empty(max(slots, 1), dtype=torch.int32, device=dev)
+    ll = torch.empty(max(slots, 1), dtype=torch.float64, device=dev)
+    mask = torch.empty(int(off[-1]), dtype=torch.uint8, device=dev) if return_mask else None
+    L.check(lib.lkb_bls_stats(L.ptr(t), L.ptr(y), L.ptr(dy), L.ptr(off), B, L.ptr(period), L.ptr(duration),
+                              L.ptr(transit_time), L.ptr(toff), L.ptr(stats), L.ptr(first), L.ptr(n_tr), L.ptr(cnt),
+                              L.ptr(ll), L.ptr(mask), L.ptr(status), L.MEM_DEVICE, _stream_ptr()))
+    res = dict(stats=stats, transit_first=first, transit_n=n_tr, per_transit_count=cnt[:slots],
+               per_transit_log_likelihood=ll[:slots], status=status, offsets=off, transit_offsets=toff)
+    if return_mask:
+        res["in_transit"] = mask
+    return res
+
+
 def bls_bin_index(t_rel, min_t, period, bin_duration):
     lib = L.load()
     t_rel = np.ascontiguousarray(t_rel, dtype=np.float64)

@@ -662,6 +662,13 @@ class BoxLeastSquaresPeriodogram(Periodogram):
         w = np.linalg.solve(np.dot(A.T, A * ivar[:, None]), np.dot(A.T, y * ivar))
         mod = np.dot(A, w)
         sin_ll = -0.5 * np.sum((y - mod) ** 2 * ivar)
+        return self._stats_dict(tstart, transit_times, counts, lls, depth, depth_phase, depth_half, depth_odd,
+                                depth_even, np.sqrt(np.sum(w[:2] ** 2)), sin_ll - full_ll)
+
+    def _stats_dict(self, tstart, transit_times, counts, lls, depth, depth_phase, depth_half, depth_odd, depth_even,
+                    harmonic_amplitude, harmonic_delta_log_likelihood):
+        """The dict compute_stats returns: `transit_times` measured from `tstart` (the first cadence), the depths as
+        (value, error) pairs in flux units."""
         yu = self.flux.unit
         q = lambda pair: (Quantity(pair[0], yu), Quantity(pair[1], yu))
         return dict(
@@ -673,9 +680,107 @@ class BoxLeastSquaresPeriodogram(Periodogram):
             depth_half=q(depth_half),
             depth_odd=q(depth_odd),
             depth_even=q(depth_even),
-            harmonic_amplitude=Quantity(np.sqrt(np.sum(w[:2] ** 2)), yu),
-            harmonic_delta_log_likelihood=sin_ll - full_ll,
+            harmonic_amplitude=Quantity(harmonic_amplitude, yu),
+            harmonic_delta_log_likelihood=harmonic_delta_log_likelihood,
         )
+
+    # -- batched follow-ups: many periodograms, one candidate each, one GPU call (K10) --------------------------------
+    @staticmethod
+    def _batch_candidates(periodograms, period, duration, transit_time):
+        """Per-periodogram (period, duration, transit_time) as float arrays [B]: None takes each periodogram's values
+        at max power (one warning per call, as _defaults words it), a scalar is broadcast, a sequence has B values."""
+        B = len(periodograms)
+        out = []
+        for name, val, attr in (("period", period, "period_at_max_power"),
+                                ("duration", duration, "duration_at_max_power"),
+                                ("transit time", transit_time, "transit_time_at_max_power")):
+            if val is None:
+                vals = [getattr(pg, attr) for pg in periodograms]
+                log.warning("No {0} specified. Using {0} at max power".format(name))
+            elif np.ndim(getattr(val, "value", val)) == 0:
+                vals = [val] * B
+            else:
+                vals = list(val)
+                if len(vals) != B:
+                    raise ValueError("{} has {} values for {} periodograms".format(name, len(vals), B))
+            out.append(np.array([float(np.asarray(getattr(x, "value", x))) for x in vals], dtype=np.float64))
+        return out
+
+    @staticmethod
+    def _batch_call(periodograms, period, duration, transit_time, return_mask):
+        from . import engine
+        pgs = list(periodograms)
+        for b, pg in enumerate(pgs):
+            if len(pg.time) == 0:
+                raise ValueError("periodogram {} ({!r}) has no cadences".format(b, pg))
+        per, dur, tt = BoxLeastSquaresPeriodogram._batch_candidates(pgs, period, duration, transit_time)
+        times = [np.asarray(pg.time.value, dtype=np.float64) for pg in pgs]
+        fluxes = [np.asarray(pg.flux.value, dtype=np.float64) for pg in pgs]
+        dys = [getattr(pg, "_dy", None) for pg in pgs]
+        if all(d is None for d in dys):
+            dys = None
+        else:          # unit weights where a periodogram has no flux_err: 1 / 1**2 is exactly what compute_stats uses
+            dys = [np.ones(len(t)) if d is None else np.asarray(d, dtype=np.float64) for t, d in zip(times, dys)]
+        res = engine.bls_stats(times, fluxes, dys, per, dur, tt, return_mask=return_mask)
+        return pgs, times, per, tt, res
+
+    @staticmethod
+    def compute_stats_batch(periodograms, period=None, duration=None, transit_time=None):
+        """``[pg.compute_stats(period, duration, transit_time) for pg in periodograms]`` in one GPU call (K10).
+
+        Each of period, duration and transit_time may be None (each periodogram's value at max power), a scalar for
+        all, or a sequence with one value per periodogram.  The masks, transit times and per-transit counts equal the
+        loop's exactly; the depths, errors and log-likelihoods agree to rounding (the GPU sums in another order).
+        Raises numpy.linalg.LinAlgError for the first periodogram whose sine fit is singular, as the loop would."""
+        from . import _lib
+        pgs = list(periodograms)
+        if not pgs:
+            return []
+        pgs, times, per, tt, res = BoxLeastSquaresPeriodogram._batch_call(pgs, period, duration, transit_time, False)
+        bad = np.flatnonzero(res["status"] == _lib.E_SINGULAR)
+        if len(bad):
+            raise np.linalg.LinAlgError("Singular matrix (periodogram {}: {!r})".format(bad[0], pgs[bad[0]]))
+        toff = res["transit_offsets"]
+        out = []
+        for b, pg in enumerate(pgs):
+            s = res["stats"][b]
+            tstart = times[b][0]
+            n = int(res["transit_n"][b])
+            if n > 0:
+                first = res["transit_first"][b]
+                transit_times = per[b] * np.arange(first, first + n) + (tt[b] - tstart)
+                counts = res["per_transit_count"][toff[b]:toff[b] + n].astype(int)
+                lls = res["per_transit_log_likelihood"][toff[b]:toff[b] + n].copy()
+            else:
+                transit_times, counts, lls = np.zeros(0), np.zeros(0, dtype=int), np.zeros(0)
+            out.append(pg._stats_dict(tstart, transit_times, counts, lls, (s[0], s[1]), (s[8], s[9]), (s[6], s[7]),
+                                      (s[2], s[3]), (s[4], s[5]), s[10], s[11]))
+        return out
+
+    @staticmethod
+    def get_transit_mask_batch(periodograms, period=None, duration=None, transit_time=None):
+        """``[pg.get_transit_mask(period, duration, transit_time) for pg in periodograms]`` in one GPU call (K10);
+        arguments as for compute_stats_batch.  get_transit_mask is `model != median(model)` for the two-valued box
+        model (y_in in transit, y_out elsewhere), so it follows from the in-transit mask and count: with fewer than
+        half the cadences in transit the median is y_out, with more it is y_in, with exactly half it is their mean."""
+        pgs = list(periodograms)
+        if not pgs:
+            return []
+        pgs, times, per, tt, res = BoxLeastSquaresPeriodogram._batch_call(pgs, period, duration, transit_time, True)
+        off = res["offsets"]
+        out = []
+        for b in range(len(pgs)):
+            s = res["stats"][b]
+            n, n_in, y_in, y_out = len(times[b]), int(s[14]), s[12], s[13]
+            m_in = res["in_transit"][off[b]:off[b + 1]]
+            if 2 * n_in < n:
+                med = y_out
+            elif 2 * n_in > n:
+                med = y_in
+            else:
+                med = np.mean([y_in, y_out])
+            out.append(np.where(m_in, y_in != med, y_out != med))
+        return out
 
     def get_transit_model(self, period=None, duration=None, transit_time=None):
         """Box transit model (periodogram.py:1231-1274; astropy BoxLeastSquares.model)."""
