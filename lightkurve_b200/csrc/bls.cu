@@ -35,6 +35,23 @@
 
 namespace lkb {
 
+// Paths a search can take.  LKB_BLS_OBSERVE(path) marks where the kernel takes one; it expands to nothing here, and
+// tests/native/bls_emu_driver.cpp, which runs this file on the CPU, defines it to count, so that each emulated test
+// case can assert that it reached the path it was written for.  Counted per (light curve, period) for the first
+// three, per warp step for WRAP3, per sample for SLOW_DIV and per boundary for EXACT_WALK.
+enum BlsPath {
+  BLS_PATH_CADENCE = 0,   // histogram built from the cadences (bls_warp_bin)
+  BLS_PATH_BOUNDARY,      // histogram built from bin boundaries (table lookup + run sums)
+  BLS_PATH_GHIST,         // histogram in the global workspace
+  BLS_PATH_WRAP3,         // a warp's 32 cadences span three or more monotone pieces (two or more period wraps)
+  BLS_PATH_SLOW_DIV,      // bls_bin_warp: a sample near a bin edge takes the IEEE division
+  BLS_PATH_EXACT_WALK,    // boundary path: a cadence near the boundary, exact walk with bls_cycle_bin
+  BLS_PATH_COUNT
+};
+#ifndef LKB_BLS_OBSERVE
+#define LKB_BLS_OBSERVE(path) ((void)0)
+#endif
+
 // (int)(r / bd) with the IEEE division replaced, on the fast path, by a reciprocal multiply whose
 // result is PROVEN equal: k = trunc(r * (1/bd)); rem = fma(-k, bd, r) is the (once rounded) remainder;
 // if 0 <= rem < bd_safe = bd * (1 - (kmax + 2) 2^-51) with kmax >= k, the real quotient lies in
@@ -58,7 +75,10 @@ __device__ __forceinline__ int bls_bin_warp(double x, bool valid, double period,
   const double rem = fma(-k, bd, r);
   const bool slow = valid && !(rem >= 0.0 && rem < bd_safe);
   if (__any_sync(0xffffffffu, slow)) {
-    if (slow) k = trunc(bls_div_slow(r, bd));
+    if (slow) {
+      LKB_BLS_OBSERVE(BLS_PATH_SLOW_DIV);
+      k = trunc(bls_div_slow(r, bd));
+    }
   }
   return valid ? (int)k + 1 : -1;
 }
@@ -224,6 +244,7 @@ __device__ __forceinline__ void bls_warp_bin(int key, double2 c_i, double2 c_nex
     // split into monotone pieces so that equal keys are contiguous within a piece
     const int piece = __popc(wrapmask & le);
     const int npieces = __popc(wrapmask) + 1;
+    if (npieces > 2 && lane == 0) LKB_BLS_OBSERVE(BLS_PATH_WRAP3);
     for (int q = 0; q < npieces; ++q) {
       if (tail && piece == q) { double2 c = h[key]; c.x += vy; c.y += vi; h[key] = c; }
       __syncwarp();
@@ -363,7 +384,7 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
                   double* __restrict__ o_power, double* __restrict__ o_depth, double* __restrict__ o_depth_err,
                   double* __restrict__ o_duration, double* __restrict__ o_ttime, double* __restrict__ o_snr,
                   double* __restrict__ o_ll, int32_t* __restrict__ o_bins) {
-  extern __shared__ __align__(16) unsigned char bls_smem[];
+  LKB_DYN_SMEM(unsigned char, bls_smem);
   double* s_t = reinterpret_cast<double*>(bls_smem);              // sample times of the tile
   double2* s_c = reinterpret_cast<double2*>(s_t + BLS_TILE);      // BLS_TILE + 1 exclusive prefix sums
   double2* s_scr = s_c + BLS_TILE + 1;                            // BLS_WARPS * 32
@@ -415,6 +436,7 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
 
   if (use_fast) {
     if (!active) return;
+    if (lane == 0) LKB_BLS_OBSERVE(BLS_PATH_BOUNDARY);
     __syncwarp();
     const double* x = trel + o;
     const double2* c = fast.cpre + o + b;
@@ -457,6 +479,7 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
         if (e > n) e = (int)n;                   // (the clamped candidates repeat the last cadence)
         const double tol = 1.0e-13 * (xb + per);
         if ((e < n && xhi - xb <= tol) || xb - xlo <= tol) {
+          LKB_BLS_OBSERVE(BLS_PATH_EXACT_WALK);
           e = e0;
           while (e < n) {
             int qi, ki;
@@ -507,7 +530,9 @@ bls_search_kernel(const double* __restrict__ trel, const double* __restrict__ wy
       }
     }
     if (!active) return;
+    if (lane == 0) LKB_BLS_OBSERVE(BLS_PATH_CADENCE);
   }
+  if (GHIST && lane == 0) LKB_BLS_OBSERVE(BLS_PATH_GHIST);
   __syncwarp();
   bls_finish_warp(h, n_bins, oversample, s_scr + warp * 32, lane, li, dur_bins, D, bin_duration, objective, per,
                   inv_per, (int64_t)b * out_stride + p, o_power, o_depth, o_depth_err, o_duration, o_ttime, o_snr, o_ll, o_bins);
@@ -523,7 +548,7 @@ int bls_bin_index(const double* t_rel, int64_t N, double min_t, double period, d
   int32_t* d_i = nullptr;
   LKB_TRY(stage_in<double>(mem, WS_IN0, t_rel, N, &d_t, st));
   LKB_TRY(stage_out_alloc<int32_t>(mem, WS_OUT0, ind, N, &d_i));
-  bls_bin_index_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(d_t, N, min_t, period, bin_duration, d_i);
+  LKB_LAUNCH((unsigned)((N + 255) / 256), 256, st, bls_bin_index_kernel)(d_t, N, min_t, period, bin_duration, d_i);
   LKB_LAUNCH_CHECK();
   LKB_TRY(stage_out_copy<int32_t>(mem, ind, d_i, N, st));
   if (mem == LKB_MEM_HOST) LKB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -636,7 +661,7 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
 
   double2* d_cpre = nullptr;
   LKB_TRY(ws_get_t<double2>(WS_H, total + B, &d_cpre));
-  bls_prep_kernel<<<B, 256, 0, st>>>(d_t, d_y, d_dy, d_off, d_trel, d_wy, d_iv, d_cpre, d_info);
+  LKB_LAUNCH(B, 256, st, bls_prep_kernel)(d_t, d_y, d_dy, d_off, d_trel, d_wy, d_iv, d_cpre, d_info);
   LKB_LAUNCH_CHECK();
 
   // boundary path set-up: per-light-curve lookup tables "first cadence at or after j * delta", built per table
@@ -666,8 +691,7 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
   }
   // search launches: CTA descriptors of every table group, uploaded once
   BlsPlanLimits lim;
-  static const int ghist_bins = getenv("LKB_BLS_GHIST_BINS") ? atoi(getenv("LKB_BLS_GHIST_BINS")) : -1;
-  lim.ghist_bins = ghist_bins;
+  if (const char* e = getenv("LKB_BLS_GHIST_BINS")) lim.ghist_bins = atoi(e);
   if (getenv("LKB_BLS_HIST_CAP_MB")) lim.hist_cap = (size_t)atoll(getenv("LKB_BLS_HIST_CAP_MB")) << 20;
   BlsPlan plan;
   std::vector<size_t> group_launch(groups.size() + 1, 0);
@@ -717,8 +741,8 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
     int64_t nT_max = 0;
     for (int b = g.b0; b < g.b1; ++b) nT_max = std::max(nT_max, h_to[b + 1] - h_to[b]);
     const unsigned gxT = (unsigned)min((int64_t)64, (nT_max + 255) / 256);
-    bls_table_kernel<<<dim3(gxT ? gxT : 1, (unsigned)(g.b1 - g.b0)), 256, 0, st>>>(d_trel, d_off, d_to + gi, g.b0,
-                                                                                   fast.delta, d_tab);
+    LKB_LAUNCH(dim3(gxT ? gxT : 1, (unsigned)(g.b1 - g.b0)), 256, st, bls_table_kernel)(d_trel, d_off, d_to + gi, g.b0,
+                                                                                        fast.delta, d_tab);
     fast.tab = d_tab;
     fast.tab_offsets = d_to + gi;
   };
@@ -731,15 +755,17 @@ int bls_power(const double* t, const double* y, const double* dy, const int64_t*
       const BlsLaunch& l = plan.launch[li];
       const unsigned gx = (unsigned)(l.cta_end - l.cta_begin);
       if (l.ghist)
-        bls_search_kernel<true><<<gx, l.W * 32, l.smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per,
-                                                              d_cta + l.cta_begin, out_stride, d_durbins, D,
-                                                              bin_duration, oversample, objective, l.stride, g_hist,
-                                                              fast, o0, o1, o2, o3, o4, o5, o6, ob);
+        LKB_LAUNCH_SMEM(gx, l.W * 32, l.smem, st, bls_search_kernel<true>)(d_trel, d_wy, d_iv, d_off, d_info, d_per,
+                                                                           d_cta + l.cta_begin, out_stride, d_durbins,
+                                                                           D, bin_duration, oversample, objective,
+                                                                           l.stride, g_hist, fast, o0, o1, o2, o3, o4,
+                                                                           o5, o6, ob);
       else
-        bls_search_kernel<false><<<gx, l.W * 32, l.smem, st>>>(d_trel, d_wy, d_iv, d_off, d_info, d_per,
-                                                               d_cta + l.cta_begin, out_stride, d_durbins, D,
-                                                               bin_duration, oversample, objective, l.stride, nullptr,
-                                                               fast, o0, o1, o2, o3, o4, o5, o6, ob);
+        LKB_LAUNCH_SMEM(gx, l.W * 32, l.smem, st, bls_search_kernel<false>)(d_trel, d_wy, d_iv, d_off, d_info, d_per,
+                                                                            d_cta + l.cta_begin, out_stride, d_durbins,
+                                                                            D, bin_duration, oversample, objective,
+                                                                            l.stride, nullptr, fast, o0, o1, o2, o3,
+                                                                            o4, o5, o6, ob);
     }
     LKB_LAUNCH_CHECK();
   }

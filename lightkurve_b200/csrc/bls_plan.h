@@ -214,7 +214,10 @@ struct BlsTableGroup {
 };
 
 constexpr double BLS_TABLE_MAX_CELLS = 6.0e7;
-constexpr int64_t BLS_TABLE_BUDGET = (int64_t)1 << 28;
+// (a test build may define a small budget to get several table groups from small inputs)
+#ifndef BLS_TABLE_BUDGET
+#define BLS_TABLE_BUDGET ((int64_t)1 << 28)
+#endif
 
 // shared == true: the batch-wide rule of the shared-grid entry (one group; no table for any light curve when
 // one of them exceeds BLS_TABLE_MAX_CELLS or the batch exceeds the budget).  shared == false: groups of

@@ -20,6 +20,9 @@
 #define __shared__ static
 #ifndef __launch_bounds__
 #define __launch_bounds__(...)
+#endif
+#ifndef __noinline__
+#define __noinline__ __attribute__((noinline))
 #endif          // one block at a time: a function-local static IS the block's shared memory
 
 namespace lkb_emu {
@@ -48,6 +51,7 @@ struct Block {
   std::vector<Barrier> warp;
   std::vector<unsigned long long> scratch;      // 32 slots per warp
   std::vector<unsigned char> alive;             // per thread
+  std::vector<int> vote;                        // per thread (__syncthreads_and)
   std::vector<unsigned long long> dyn;          // dynamic shared memory of the block
 };
 
@@ -85,6 +89,7 @@ void lkb_emu::Launcher<F>::operator()(Args... args) {
         for (int w = 0; w < nwarps; ++w) blk.warp[w].reset(std::min(32, nthreads - 32 * w));
         blk.scratch.assign((size_t)nwarps * 32, 0ull);
         blk.alive.assign(nthreads, 1);
+        blk.vote.assign(nthreads, 1);
         blk.dyn.assign(smem_bytes / 8 + 2, 0ull);
         std::vector<std::thread> th;
         th.reserve(nthreads);
@@ -115,6 +120,17 @@ void lkb_emu::Launcher<F>::operator()(Args... args) {
 
 // ---- device built-ins ------------------------------------------------------------------------------------
 inline void __syncthreads() { lkb_emu::t_block->all.wait(); }
+// the AND of `pred` over the block's threads that have not returned
+inline int __syncthreads_and(int pred) {
+  lkb_emu::Block* b = lkb_emu::t_block;
+  b->vote[lkb_emu::t_tid] = pred ? 1 : 0;
+  b->all.wait();
+  int out = 1;
+  for (size_t t = 0; t < b->vote.size(); ++t)
+    if (b->alive[t] && !b->vote[t]) out = 0;
+  b->all.wait();
+  return out;
+}
 
 template <typename T>
 inline T __shfl_xor_sync(unsigned, T v, int lane_mask) {
@@ -180,6 +196,7 @@ inline unsigned __ballot_sync(unsigned, int pred) {
   b->warp[w].wait();
   return out;
 }
+inline int __any_sync(unsigned mask, int pred) { return __ballot_sync(mask, pred) != 0; }
 inline unsigned __match_any_sync(unsigned, int value) {
   lkb_emu::Block* b = lkb_emu::t_block;
   const int t = lkb_emu::t_tid, w = t / 32, lane = t % 32;
