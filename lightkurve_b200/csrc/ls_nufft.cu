@@ -1255,8 +1255,22 @@ nufft_lowrows_ragged_kernel(const double* __restrict__ t, const float* __restric
 // disguise: j f sits near a multiple of the sampling rate of a near-regular cadence (a TESS 2-min light curve: 720 / d,
 // which the harmonics of a grid up to the Nyquist frequency reach), the normal matrix cancels like that of
 // f * baseline <= 2, and the fp32 sums miss the tolerance there (emulated 2-min light curves: up to 300x within one bin
-// of 720 / d).  Such bins take the direct fp64 sums, in this thread; irregular cadences never get near the limit.
+// of 720 / d).  Such bins take the direct fp64 sums, in this thread.  Irregular cadences reach the limit only by chance,
+// with probability ~exp(-N / 16) per harmonic and bin: never at N >= 300, a fifth of the bins or more at N ~ 40.
 constexpr double LS_CHI2_COHERENT = 0.25;
+// Paths of the multi-term NUFFT periodogram.  LKB_CHI2_OBSERVE(path) marks where one is taken; it expands to nothing
+// here, and tests/native/nufft_chi2_emu_driver.cpp, which runs this file on the CPU, defines it to count, so that each
+// emulated case can assert that it reached the paths it was written for.  Counted per (light curve, bin) for the
+// first two and per group of light curves for the last.
+enum Chi2Path {
+  CHI2_PATH_COHERENT = 0,   // nufft2_finish_chi2_ragged_kernel: a nearly coherent window sum, bin recomputed in fp64
+  CHI2_PATH_LOW_ROW,        // nufft_lowrows_chi2_ragged_kernel: f * baseline <= LS_LOWF_CYCLES, direct fp64 sums
+  CHI2_PATH_GROUP,          // ls_nufft_ragged_v2: one group of light curves through the fine-grid buffers
+  CHI2_PATH_COUNT
+};
+#ifndef LKB_CHI2_OBSERVE
+#define LKB_CHI2_OBSERVE(path) ((void)0)
+#endif
 template <int NT>
 __global__ void __launch_bounds__(256)
 nufft2_finish_chi2_ragged_kernel(const float2* __restrict__ Zn, int p, const float2* __restrict__ Zwn, int p2,
@@ -1294,6 +1308,7 @@ nufft2_finish_chi2_ragged_kernel(const float2* __restrict__ Zn, int p, const flo
 #pragma unroll
   for (int j = 0; j < 2 * NT; ++j) coherent |= d.C[j] * d.C[j] + d.S[j] * d.S[j] >= LS_CHI2_COHERENT * LS_CHI2_COHERENT * Nd * Nd;
   if (coherent) {
+    LKB_CHI2_OBSERVE(CHI2_PATH_COHERENT);
     d.zero();
     for (int64_t i = 0; i < n; ++i) chi2_add<NT>(d, (double)y[poff[b] + i], fr * t[poff[b] + i]);
   }
@@ -1324,6 +1339,7 @@ nufft_lowrows_chi2_ragged_kernel(const double* __restrict__ t, const float* __re
   for (int64_t i = lane; i < n; i += 32) chi2_add<NT>(d, (double)y[po + i], fr * t[po + i]);
   chi2_warp_reduce<NT>(d);
   if (lane == 0) {
+    LKB_CHI2_OBSERVE(CHI2_PATH_LOW_ROW);
     double pw;
     chi2_solve<NT>(d, (double)n, ysum[b], pw, nullptr);
     power[b * F + k] = ls_normalize(pw, (double)n, normalization, norm_scale ? norm_scale[b] : 1.0);
@@ -1395,6 +1411,7 @@ int ls_nufft_ragged_v2(const double* d_t, const float* d_y, const int64_t* d_off
   const int nk2 = (int)(kmax >> (p - 1 - V2_PB)) + 1, nk2w = (int)((2 * kmax) >> (p2 - 1 - V2_PB)) + 1;
   prof_begin(st);
   for (int b0 = 0; b0 < B; b0 += group) {
+    LKB_CHI2_OBSERVE(CHI2_PATH_GROUP);
     const int Bg = std::min(group, B - b0);
     const int64_t *off_g = d_off + b0, *po_g = d_po + b0;
     double span_min = 1e300;
@@ -1623,7 +1640,9 @@ int ls_nufft_chi2_ragged_launch(const double* d_t, const float* d_y, const int64
   int64_t k0 = 0;
   LKB_TRY(ragged_grid_check(B, h_span, f0, df, &k0));
   const int64_t kmax = (int64_t)nterms * (k0 + F);
-  const int p = fine_log2(kmax), p2 = fine_log2(2 * kmax);
+  // both grids at least 2^V2R_P_MIN cells, as for the single-term transforms (single_term_log2): a small grid takes the
+  // v2 transform instead of being refused; sigma = min(2, grid_sigma) keeps the kernel width and shape
+  const int p = std::max(fine_log2(kmax), V2R_P_MIN), p2 = std::max(fine_log2(2 * kmax), V2R_P_MIN);
   if (p2 > V2R_P_MAX || fft_mode(p) != 3 || fft_mode(p2) != 3) {
     set_error("NUFFT (ragged chi2): fine grids of 2^%d / 2^%d cells are outside the v2 transform's range", p, p2);
     return LKB_E_UNSUPPORTED;
