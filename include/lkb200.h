@@ -287,6 +287,33 @@ int lkb_regress_ex(const double* X, int x_batched, const double* y, const double
                    double* coeff, double* model, uint8_t* outlier_mask, int32_t* status_out, double* coeff_cov,
                    int mem, void* stream, int prior_batched, int flags);
 
+/* ---- sigma clip and CDPP (K11, K12) ---------------------------------------- */
+/* K11: replaces the host loop of LightCurve.remove_outliers, lightcurve.py:1429-1549 (astropy.stats.sigma_clip
+ * (x, sigma_lower=, sigma_upper=, maxiters=).mask with cenfunc="median", stdfunc="std").  One CTA per light curve
+ * runs every round: non-finite values are masked from the start, a round clips x < med - sigma_lower * std or
+ * x > med + sigma_upper * std of the values still kept (std with ddof 0), the mask is cumulative, and the loop stops
+ * when a round clips nothing or after maxiters rounds (maxiters < 0: until then - maxiters=None).
+ *   x            [offsets[B]] fp64; offsets int64 [B + 1] HOST memory in both modes
+ *   mask_out     uint8 [offsets[B]], 1 = clipped or non-finite         (each output may be NULL)
+ *   center_out   [B] median of the kept values (NaN when none is kept)
+ *   std_out      [B] their standard deviation, ddof 0
+ *   n_kept_out   int64 [B] */
+int lkb_sigma_clip(const double* x, const int64_t* offsets, int B, double sigma_lower, double sigma_upper,
+                   int maxiters, uint8_t* mask_out, double* center_out, double* std_out, int64_t* n_kept_out,
+                   int mem, void* stream);
+/* K4 + K11 + K12: replaces LightCurve.estimate_cdpp, lightcurve.py:1764-1833, for D transit durations at once:
+ * flatten(window_length=savgol_window, polyorder=savgol_polyorder) with break_tolerance 5, niters 3, sigma 3 and no
+ * mask (polyorder >= window is clamped as lkb_flatten clamps it); remove_outliers(sigma) (maxiters 5); normalize
+ * ("ppm"); then cdpp[b, d] = std(running_mean(normalized flux, durations[d])), ddof 0, where the running means are
+ * the n_kept - w + 1 means over w = min(durations[d], n_kept) consecutive kept cadences (array positions, not time).
+ * NaN for a light curve with no kept cadence.  The flattened flux stays on the device.
+ *   time, flux   [offsets[B]] fp64; offsets int64 [B + 1] and durations int32 [D] are HOST memory in both modes
+ *   durations    each >= 1, else LKB_E_ARG
+ *   cdpp_out     [B, D] fp64, ppm */
+int lkb_cdpp(const double* time, const double* flux, const int64_t* offsets, int B,
+             const int32_t* durations, int D, int savgol_window, int savgol_polyorder, double sigma,
+             double* cdpp_out, int mem, void* stream);
+
 /* ---- batched order statistics (K6) ---------------------------------------- */
 /* nanmedian and nanstd (ddof=0) per light curve: np.nanmedian / np.nanstd as used by
  * normalize (lightcurve.py:1253-1254) and flatten (:1003-1005). out_median/out_std [B]. */

@@ -69,6 +69,8 @@ SIGNATURES = {
                                c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_savgol_tables": (c_int, [c_int, c_int, c_vp, c_vp]),
     "lkb_nanmedian_std": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp]),
+    "lkb_sigma_clip": (c_int, [c_vp, c_vp, c_int, c_dbl, c_dbl, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
+    "lkb_cdpp": (c_int, [c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_dbl, c_vp, c_int, c_vp]),
     "lkb_pg_logmedian": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_dbl, c_vp, c_int, c_vp]),
     "lkb_acf_windows": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_nccl_version": (c_int, []),

@@ -4,9 +4,14 @@ over the whole collection in ONE kernel launch sequence.  Their contract is "ide
 ``[lc.method(...) for lc in collection]``" - the per-light-curve preparation code is literally
 the same functions (``LombScarglePeriodogram._prepare`` etc.); only the device call is batched.
 """
+import logging
+import math
+
 import numpy as np
 
 from .lightcurve import LightCurve
+
+log = logging.getLogger(__name__)
 
 __all__ = ["Collection", "LightCurveCollection"]
 
@@ -145,6 +150,65 @@ class LightCurveCollection(Collection):
         if return_trend:
             return LightCurveCollection(flats), LightCurveCollection(trends)
         return LightCurveCollection(flats)
+
+    def remove_outliers(self, sigma=5.0, sigma_lower=None, sigma_upper=None, return_mask=False, column="flux",
+                        maxiters=5, **kwargs):
+        """Batched ``LightCurve.remove_outliers``: equal to ``[lc.remove_outliers(...) for lc in collection]``, with
+        every clip round of every light curve in one GPU call (K11, ``engine.sigma_clip``).  ``maxiters=None`` clips
+        until a round clips nothing.  Returns a LightCurveCollection and, with ``return_mask``, the list of boolean
+        masks (True = removed).  Of astropy's further ``sigma_clip`` keywords only the defaults ``cenfunc="median"``
+        and ``stdfunc="std"`` are accepted; anything else raises, as in the single-curve method."""
+        from . import engine
+        if kwargs.pop("cenfunc", "median") not in ("median", np.median, np.nanmedian) or \
+                kwargs.pop("stdfunc", "std") not in ("std", np.std, np.nanstd):
+            raise NotImplementedError("remove_outliers(): only cenfunc='median' and stdfunc='std' run on the GPU kernel")
+        if kwargs:
+            raise TypeError("remove_outliers(): unsupported sigma_clip keyword(s) %s" % sorted(kwargs))
+        lo_s = sigma if sigma_lower is None else sigma_lower
+        hi_s = sigma if sigma_upper is None else sigma_upper
+        # the single-curve loop runs `while it < maxiters`: a fractional maxiters rounds up, a negative one clips nothing
+        mi = -1 if maxiters is None else max(0, math.ceil(maxiters))
+        cols = []
+        for lc in self.data:
+            col = getattr(lc, column)
+            cols.append(np.array(getattr(col, "value", col), dtype=np.float64))
+        masks = engine.sigma_clip(cols, float(lo_s), float(hi_s), mi)["mask"] if cols else []
+        out = LightCurveCollection([lc[~m] for lc, m in zip(self.data, masks)])
+        if return_mask:
+            return out, [np.array(m, dtype=bool) for m in masks]
+        return out
+
+    def estimate_cdpp(self, transit_duration=13, savgol_window=101, savgol_polyorder=2, sigma=5.0):
+        """Batched ``LightCurve.estimate_cdpp``: the Savitzky-Golay CDPP of every light curve in ppm, from one GPU call
+        (K4 flatten, K11 remove_outliers, K12 normalize and running-mean scatter; ``engine.cdpp``) in which the
+        flattened flux never leaves the device.  Returns a Quantity of shape [B].  ``transit_duration`` may also be a
+        sequence of ints: the CDPP at each of them, shape [B, D], from the same call.
+
+        Equals ``[lc.estimate_cdpp(...) for lc in collection]`` for float64 flux.  Float32 flux is worked in float64
+        throughout, which equals the loop on a float64 copy; the single-curve method instead keeps float32 through
+        ``normalize`` and the cumulative sum of ``running_mean``, so its result differs from this one by that float32
+        rounding."""
+        from . import engine
+        from . import units as u
+        seq = not isinstance(transit_duration, int) and np.ndim(transit_duration) == 1
+        durs = list(transit_duration) if seq else [transit_duration]
+        for d in durs:
+            if not (isinstance(d, int) or (seq and isinstance(d, np.integer))):
+                raise ValueError(
+                    "transit_duration must be an integer in units "
+                    "number of cadences, got {}.".format(d)
+                )
+        if savgol_polyorder >= savgol_window:
+            savgol_polyorder = savgol_window - 1
+            log.warning("polyorder must be smaller than window_length, "
+                        "using polyorder={}.".format(savgol_polyorder))
+        if not self.data:
+            res = np.zeros((0, len(durs)))
+        else:
+            times = [np.asarray(lc.time.value, dtype=np.float64) for lc in self.data]
+            fluxes = [np.asarray(lc.flux.value, dtype=np.float64) for lc in self.data]
+            res = engine.cdpp(times, fluxes, np.asarray(durs, dtype=np.int64), savgol_window, savgol_polyorder, sigma)
+        return u.Quantity(res if seq else res[:, 0], u.ppm)
 
     def stitch(self, corrector_func=lambda x: x.normalize()):
         """Concatenate the light curves (collections.py:196-230)."""

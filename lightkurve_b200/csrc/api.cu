@@ -234,6 +234,10 @@ int underfit_metric(const double*, int, const double*, int, int64_t, const int64
                     double*, int, cudaStream_t);
 int overfit_terms(const float*, const float*, const float*, const int64_t*, int, int64_t, int, int32_t*, double*,
                   double*, int, cudaStream_t);
+int sigma_clip(const double*, const int64_t*, int, double, double, int, uint8_t*, double*, double*, int64_t*, int,
+               cudaStream_t);
+int cdpp(const double*, const double*, const int64_t*, int, const int32_t*, int, int, int, double, double*, int,
+         cudaStream_t);
 
 }  // namespace lkb
 
@@ -463,6 +467,21 @@ int lkb_nanmedian_std(const double* x, const int64_t* offsets, int B, double* ou
                       void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return nanmedian_std(x, offsets, B, out_median, out_std, mem, (cudaStream_t)stream);
+}
+
+int lkb_sigma_clip(const double* x, const int64_t* offsets, int B, double sigma_lower, double sigma_upper,
+                   int maxiters, uint8_t* mask_out, double* center_out, double* std_out, int64_t* n_kept_out,
+                   int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return sigma_clip(x, offsets, B, sigma_lower, sigma_upper, maxiters, mask_out, center_out, std_out, n_kept_out, mem,
+                    (cudaStream_t)stream);
+}
+
+int lkb_cdpp(const double* time, const double* flux, const int64_t* offsets, int B, const int32_t* durations, int D,
+             int savgol_window, int savgol_polyorder, double sigma, double* cdpp_out, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return cdpp(time, flux, offsets, B, durations, D, savgol_window, savgol_polyorder, sigma, cdpp_out, mem,
+              (cudaStream_t)stream);
 }
 
 int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_lo, const int32_t* win_hi, int W,

@@ -735,6 +735,85 @@ def nanmedian_std(arrays):
     return med, sd
 
 
+def sigma_clip(arrays, sigma_lower=3.0, sigma_upper=3.0, maxiters=5, offsets=None):
+    """K11.  astropy.stats.sigma_clip(x, sigma_lower=, sigma_upper=, maxiters=).mask (cenfunc="median", stdfunc="std")
+    of each light curve; maxiters None (or < 0) clips until a round clips nothing.  `arrays`: a list of 1-D arrays
+    (host mode), or the concatenated CUDA float64 tensor with the host int64 CSR `offsets` [B + 1] (device mode, on
+    the current torch stream).  Returns dict(mask (host: a list of bool arrays; device: a uint8 tensor), center,
+    std (median and standard deviation, ddof 0, of the kept values), n_kept, offsets)."""
+    lib = L.load()
+    mi = -1 if maxiters is None else int(maxiters)
+    if _is_torch(arrays):
+        import torch
+        if offsets is None:
+            raise ValueError("device mode needs the host CSR `offsets`")
+        if not (arrays.is_cuda and arrays.is_contiguous() and arrays.dim() == 1 and arrays.dtype == torch.float64):
+            raise ValueError("device mode: the values must be a contiguous one-dimensional CUDA float64 tensor")
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        B = len(off) - 1
+        if B <= 0 or off[0] != 0 or np.any(np.diff(off) < 0) or off[-1] != arrays.numel():
+            raise ValueError("offsets do not describe the %d values" % arrays.numel())
+        dev = arrays.device
+        mask = torch.empty(max(int(off[-1]), 1), dtype=torch.uint8, device=dev)
+        center, sd = torch.empty(B, dtype=torch.float64, device=dev), torch.empty(B, dtype=torch.float64, device=dev)
+        nk = torch.empty(B, dtype=torch.int64, device=dev)
+        L.check(lib.lkb_sigma_clip(L.ptr(arrays), L.ptr(off), B, float(sigma_lower), float(sigma_upper), mi,
+                                   L.ptr(mask), L.ptr(center), L.ptr(sd), L.ptr(nk), L.MEM_DEVICE, _stream_ptr()))
+        return dict(mask=mask[:int(off[-1])], center=center, std=sd, n_kept=nk, offsets=off)
+    B = len(arrays)
+    if B == 0:
+        return dict(mask=[], center=np.zeros(0), std=np.zeros(0), n_kept=np.zeros(0, np.int64),
+                    offsets=np.zeros(1, np.int64))
+    x, off = _csr(arrays)
+    mask = np.empty(max(len(x), 1), dtype=np.uint8)
+    center, sd, nk = np.empty(B), np.empty(B), np.empty(B, dtype=np.int64)
+    L.check(lib.lkb_sigma_clip(L.ptr(x), L.ptr(off), B, float(sigma_lower), float(sigma_upper), mi, L.ptr(mask),
+                               L.ptr(center), L.ptr(sd), L.ptr(nk), L.MEM_HOST, None))
+    m = mask.view(bool)
+    return dict(mask=[m[off[b]:off[b + 1]] for b in range(B)], center=center, std=sd, n_kept=nk, offsets=off)
+
+
+def cdpp(times, fluxes, durations=13, savgol_window=101, savgol_polyorder=2, sigma=5.0, offsets=None):
+    """K4 + K11 + K12.  LightCurve.estimate_cdpp (lightcurve.py:1764-1833) of each light curve at each transit
+    duration (in cadences, ints >= 1): flatten, remove_outliers(sigma), normalize("ppm") and the standard deviation of
+    the running means, with the flattened flux kept on the device.  `times` / `fluxes`: lists of 1-D arrays (host
+    mode), or the concatenated CUDA float64 tensors with the host int64 CSR `offsets` [B + 1] (device mode, on the
+    current torch stream).  Returns the [B, D] ppm values (numpy, or a CUDA float64 tensor); NaN where a light
+    curve keeps no cadence."""
+    lib = L.load()
+    dur = np.ascontiguousarray(np.atleast_1d(durations), dtype=np.int32)
+    if dur.ndim != 1 or len(dur) == 0 or not np.array_equal(dur, np.atleast_1d(durations)):
+        raise ValueError("durations must be a non-empty sequence of integers")
+    D = len(dur)
+    if _is_torch(fluxes):
+        import torch
+        if offsets is None:
+            raise ValueError("device mode needs the host CSR `offsets`")
+        for name, v in (("times", times), ("fluxes", fluxes)):
+            if not (_is_torch(v) and v.is_cuda and v.is_contiguous() and v.dim() == 1 and v.dtype == torch.float64):
+                raise ValueError("device mode: %s must be a contiguous one-dimensional CUDA float64 tensor" % name)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        B = len(off) - 1
+        if B <= 0 or off[0] != 0 or np.any(np.diff(off) < 0) or off[-1] != fluxes.numel() or \
+                times.numel() != fluxes.numel():
+            raise ValueError("offsets do not describe the time and flux tensors")
+        out = torch.empty((B, D), dtype=torch.float64, device=fluxes.device)
+        L.check(lib.lkb_cdpp(L.ptr(times), L.ptr(fluxes), L.ptr(off), B, L.ptr(dur), D, int(savgol_window),
+                             int(savgol_polyorder), float(sigma), L.ptr(out), L.MEM_DEVICE, _stream_ptr()))
+        return out
+    B = len(times)
+    if B == 0:
+        return np.zeros((0, D))
+    t, off = _csr(times)
+    f, foff = _csr(fluxes)
+    if not np.array_equal(off, foff):
+        raise ValueError("time and flux lengths differ")
+    out = np.empty((B, D))
+    L.check(lib.lkb_cdpp(L.ptr(t), L.ptr(f), L.ptr(off), B, L.ptr(dur), D, int(savgol_window), int(savgol_polyorder),
+                         float(sigma), L.ptr(out), L.MEM_HOST, None))
+    return out
+
+
 def logmedian_windows(frequency, filter_width):
     """Half-open bin ranges of the reference's moving log10-frequency window (periodogram.py:267-277) for an
     ASCENDING frequency grid: window w = { i : |log10 f_i - x0_w| < filter_width }, x0 advancing by
