@@ -21,8 +21,10 @@
 //            epilogue) -> power, written in 32-byte runs (8 consecutive k1 at one k2 are 8 consecutive frequency
 //            bins); the transform itself never goes back to global memory.  The CTA that would hold row A / 2 twice
 //            takes row 0 (which mirrors onto itself) instead.
-// All tile geometry is compile-time (template parameter PA): every shared-memory offset inside the passes is
-// `runtime base + constant`.
+// All tile geometry is compile-time (template parameters PA and LOGT): every shared-memory offset inside the passes is
+// `runtime base + constant`.  A tile is 2^LOGT points, 16 per thread: the float2 kernels take 8192-point tiles (64 KB,
+// 512 threads, 2 CTAs per SM); the double2 escalation pass takes 4096-point tiles (64 KB of double2, 256 threads), so
+// that it too runs 2 CTAs per SM - at 8192 points its tiles were 128 KB, one CTA per SM, and the column kernel spilled.
 #pragma once
 #include "nufft_core.h"
 
@@ -35,7 +37,7 @@ using nufft::V2_TILE;
 constexpr int V2_LOG_TILE = 13;
 static_assert((1 << V2_LOG_TILE) == V2_TILE, "tile size");
 constexpr int V2_BC = 1 << V2_PB;
-constexpr int V2_R = V2_TILE / (2 * V2_BC);                     // rows per block of the row kernel (8)
+constexpr int V2_R = V2_TILE / (2 * V2_BC);                     // rows per block of the float2 row kernel (8)
 constexpr int V2_LSB = V2_BC + V2_BC / 16 + 1;                  // skewed line of Bc points
 // real-mode limits: Mh = 2^(p - 1) = A * Bc with 16 <= A <= 8192
 constexpr int V2R_P_MIN = V2_PB + 4 + 1, V2R_P_MAX = V2_PB + 13 + 1;
@@ -44,6 +46,9 @@ __host__ __device__ constexpr int v2_radix(int plog, int idx) {
   return (idx < plog / 4) ? 16 : ((idx == plog / 4 && (plog % 4)) ? (1 << (plog % 4)) : 0);
 }
 __host__ __device__ constexpr int v2_log2i(int r) { return r == 16 ? 4 : r == 8 ? 3 : r == 4 ? 2 : r == 2 ? 1 : 0; }
+// log2 of the tile of a transform with A = 2^pa: 8192 points in float2; 4096 in double2 (one column of 4096 points at
+// A = 4096, so A = 8192 keeps the 8192-point tile and one CTA per SM)
+__host__ __device__ constexpr int v2_log_tile(int pa, bool dbl) { return (dbl && pa <= 12) ? 12 : V2_LOG_TILE; }
 __device__ __forceinline__ int v2_skew(int a) { return a + (a >> 4); }
 // offset of input r of a butterfly (r * nb points further) in a skewed line; exact because the butterfly index is
 // either a multiple-of-16 aligned case (nb % 16 == 0) or smaller than nb <= 8
@@ -149,15 +154,16 @@ nufft2_spread_kernel(const int32_t* __restrict__ first_ge, const nufft::Cad* __r
 }
 
 // ---- in-place passes over the lines of a tile (compile-time geometry) ---------------------------------------------
-// PLOG: log2 of the line length, LS: skewed line stride, IDX / NS: pass number and the product of earlier radices.
-// nz (first pass only): line positions >= nz hold zeros that were never stored - they are not read either
-template <int PLOG, int LS, int IDX, int NS, class CT = float2>
+// PLOG: log2 of the line length, LS: skewed line stride, IDX / NS: pass number and the product of earlier radices, NT:
+// threads of the CTA (16 points each).  nz (first pass only): line positions >= nz hold zeros that were never stored -
+// they are not read either
+template <int PLOG, int LS, int IDX, int NS, class CT = float2, int NT = V2_THREADS>
 __device__ __forceinline__ void v2_pass_t(CT* buf, const CT* __restrict__ tw, int nz = 1 << 30) {
   constexpr int R = v2_radix(PLOG, IDX);
   if constexpr (R != 0) {
     constexpr int LR = v2_log2i(R), NB = 16 / R, PNB = PLOG - LR, nb = 1 << PNB;      // nb butterflies per line
-    constexpr bool WIDE = nb > V2_THREADS;           // one line, several butterflies of it per thread
-    static_assert(WIDE || (V2_THREADS % nb) == 0, "geometry");
+    constexpr bool WIDE = nb > NT;                   // one line, several butterflies of it per thread
+    static_assert(WIDE || (NT % nb) == 0, "geometry");
     // per-input offset r * nb in the skewed line: v2_in_off<nb>(r)
     const int t = (int)threadIdx.x;
     CT u[NB][R];
@@ -165,8 +171,8 @@ __device__ __forceinline__ void v2_pass_t(CT* buf, const CT* __restrict__ tw, in
 #pragma unroll
     for (int q = 0; q < NB; ++q) {
       int line, i;
-      if constexpr (WIDE) { line = 0; i = t + V2_THREADS * q; }
-      else { line = (t >> PNB) + ((V2_THREADS * q) >> PNB); i = t & (nb - 1); }
+      if constexpr (WIDE) { line = 0; i = t + NT * q; }
+      else { line = (t >> PNB) + ((NT * q) >> PNB); i = t & (nb - 1); }
       base_in[q] = line * LS + ((nb % 16 == 0) ? v2_skew(i) : i);
 #pragma unroll
       for (int r = 0; r < R; ++r)
@@ -176,8 +182,8 @@ __device__ __forceinline__ void v2_pass_t(CT* buf, const CT* __restrict__ tw, in
 #pragma unroll
     for (int q = 0; q < NB; ++q) {
       int line, i;
-      if constexpr (WIDE) { line = 0; i = t + V2_THREADS * q; }
-      else { line = (t >> PNB) + ((V2_THREADS * q) >> PNB); i = t & (nb - 1); }
+      if constexpr (WIDE) { line = 0; i = t + NT * q; }
+      else { line = (t >> PNB) + ((NT * q) >> PNB); i = t & (nb - 1); }
       const int k = i & (NS - 1);
       if constexpr (NS > 1) {
 #pragma unroll
@@ -191,7 +197,7 @@ __device__ __forceinline__ void v2_pass_t(CT* buf, const CT* __restrict__ tw, in
       for (int r = 0; r < R; ++r) buf[base_out + ((NS == 1) ? r : r * (NS + NS / 16))] = u[q][r];
     }
     __syncthreads();
-    v2_pass_t<PLOG, LS, IDX + 1, NS * R, CT>(buf, tw + ((IDX > 0) ? R * NS : 0));
+    v2_pass_t<PLOG, LS, IDX + 1, NS * R, CT, NT>(buf, tw + ((IDX > 0) ? R * NS : 0));
   }
 }
 
@@ -210,13 +216,14 @@ __device__ __forceinline__ int v2_count(const V2Count nc, int grid_y) {
 // ---- cols ---------------------------------------------------------------------------------------------------------
 // grid (Bc / TC, B).  G: pruned fine grids [B][c][n1 < n1max][j]; T: [B][c][k1][j]
 // one transform (light curve slot lc): all threads of the CTA
-template <int PA, class CT>
+template <int PA, class CT, int LOGT = V2_LOG_TILE>
 __device__ __forceinline__ void v2_cols_one(CT* buf, const CT* __restrict__ G, CT* __restrict__ T, int n1max,
                                             const CT* __restrict__ tw_a, const CT* __restrict__ t_hi,
                                             const CT* __restrict__ t_lo, const int64_t lc) {
-  constexpr int A = 1 << PA, PTC = V2_LOG_TILE - PA, TC = 1 << PTC, LS = A + A / 16 + 1, C = V2_BC / TC;
-  // one sweep of the 512 threads covers JW columns x RW rows (RW is a multiple of 16: constant skew increments)
-  constexpr int JW = TC < 32 ? TC : 32, RW = V2_THREADS / JW, CG = TC / JW;
+  constexpr int NT = (1 << LOGT) / 16;
+  constexpr int A = 1 << PA, PTC = LOGT - PA, TC = 1 << PTC, LS = A + A / 16 + 1, C = V2_BC / TC;
+  // one sweep of the NT threads covers JW columns x RW rows (RW is a multiple of 16: constant skew increments)
+  constexpr int JW = TC < NT / 16 ? TC : NT / 16, RW = NT / JW, CG = TC / JW;
   constexpr int LJW = JW == 32 ? 5 : JW == 16 ? 4 : JW == 8 ? 3 : JW == 4 ? 2 : JW == 2 ? 1 : 0;
   static_assert((1 << LJW) == JW && RW % 16 == 0, "geometry");
   const int t = (int)threadIdx.x, c = (int)blockIdx.x;
@@ -236,8 +243,8 @@ __device__ __forceinline__ void v2_cols_one(CT* buf, const CT* __restrict__ G, C
     }
   }
   __syncthreads();
-  v2_pass_t<PA, LS, 0, 1, CT>(buf, tw_a, nz);
-  CT* Tp = T + (lc * C + c) * (int64_t)V2_TILE;
+  v2_pass_t<PA, LS, 0, 1, CT, NT>(buf, tw_a, nz);
+  CT* Tp = T + (lc * C + c) * (int64_t)(1 << LOGT);
   const int ph = PA + V2_PB, pl = nufft::v2_log2_lo(ph);
   const unsigned Mmask = (1u << ph) - 1u, lmask = (1u << pl) - 1u;
 #pragma unroll
@@ -258,9 +265,18 @@ nufft2_cols_kernel(const CT* __restrict__ G, CT* __restrict__ T, int n1max, cons
   LKB_DYN_SMEM(CT, buf);
   v2_cols_one<PA, CT>(buf, G, T, n1max, tw_a, t_hi, t_lo, (int64_t)blockIdx.y);
 }
-// escalation pass (double precision): blocks stride over a device-side count of transforms
-template <int PA>
-__global__ void __launch_bounds__(V2_THREADS, 1)
+// escalation pass (double precision, tiles of 2^v2_log_tile(PA, true) points): blocks stride over a device-side count
+// of transforms.  One transform is a call, not inlined into the loop: inlined, ptxas kept the address arithmetic of
+// all 16 loads and stores live across iterations and spilled up to 584 bytes at the 128-register cap of 2 CTAs/SM.
+template <int PA, int LOGT>
+__device__ __noinline__ void v2_cols_list_one(double2* buf, const double2* __restrict__ G, double2* __restrict__ T,
+                                              int n1max, const double2* __restrict__ tw_a,
+                                              const double2* __restrict__ t_hi, const double2* __restrict__ t_lo,
+                                              const int64_t lc) {
+  v2_cols_one<PA, double2, LOGT>(buf, G, T, n1max, tw_a, t_hi, t_lo, lc);
+}
+template <int PA, int LOGT = v2_log_tile(PA, true)>
+__global__ void __launch_bounds__((1 << LOGT) / 16, LOGT < V2_LOG_TILE ? 2 : 1)
 nufft2_cols_list_kernel(const double2* __restrict__ G, double2* __restrict__ T, int n1max,
                         const double2* __restrict__ tw_a, const double2* __restrict__ t_hi,
                         const double2* __restrict__ t_lo, V2Count nc) {
@@ -268,7 +284,7 @@ nufft2_cols_list_kernel(const double2* __restrict__ G, double2* __restrict__ T, 
   const int64_t ntr = v2_count(nc, (int)gridDim.y);
   for (int64_t lc = blockIdx.y; lc < ntr; lc += gridDim.y) {
     __syncthreads();
-    v2_cols_one<PA, double2>(buf, G, T, n1max, tw_a, t_hi, t_lo, lc);
+    v2_cols_list_one<PA, LOGT>(buf, G, T, n1max, tw_a, t_hi, t_lo, lc);
   }
 }
 
@@ -321,16 +337,19 @@ __device__ __forceinline__ float v2_finish_pw(double2 g1, double2 g2, const V2FT
 
 // MODE 1: finish -> power.  MODE 2: the modes k < nk2_keep * A and their mirrors Mh - k go to Zout [B][Mh] in natural
 // order (the ragged finish kernel reads them there).  One transform (slot lc; lc_base + lc indexes fa.lcmap).
-template <int PA, int MODE, class CT>
+// Rows per half: R = 2^LOGT / (2 Bc) (8 in float2, 4 in double2); 2 R slots of Bc points fill the tile.
+template <int PA, int MODE, class CT, int LOGT = V2_LOG_TILE>
 __device__ __forceinline__ void v2_rows_one(CT* buf, const CT* __restrict__ T, const CT* __restrict__ tw_b,
                                             const V2Finish& fa, CT* __restrict__ Zout, int nk2_keep, const int64_t lc,
                                             const int lc_base, const int g) {
-  constexpr int A = 1 << PA, PTC = V2_LOG_TILE - PA, TC = 1 << PTC, R = V2_R, LS = V2_LSB, Bc = V2_BC;
+  constexpr int NT = (1 << LOGT) / 16, R = (1 << LOGT) / (2 * V2_BC), LR = v2_log2i(R);
+  constexpr int A = 1 << PA, PTC = LOGT - PA, TC = 1 << PTC, LS = V2_LSB, Bc = V2_BC;
+  static_assert((1 << LR) == R, "geometry");
   const int t = (int)threadIdx.x;
   const bool last = g == (A / (2 * R)) - 1;
   const int64_t Mh = (int64_t)1 << (PA + V2_PB);
   auto slot_k1 = [&](int s) -> int {
-    const int h = s >> 3, r = s & (R - 1);
+    const int h = s >> LR, r = s & (R - 1);
     if (h == 0) return 1 + g * R + r;
     if (last && r == 0) return 0;                    // instead of a second copy of row A / 2
     return A - (g + 1) * R + r;
@@ -338,18 +357,19 @@ __device__ __forceinline__ void v2_rows_one(CT* buf, const CT* __restrict__ T, c
   const CT* Tp = T + lc * Mh;
 #pragma unroll
   for (int u = 0; u < 16; ++u) {
-    const int e = t + V2_THREADS * u;
-    const int j = e & (TC - 1), r = (e >> PTC) & (R - 1), h = (e >> (PTC + 3)) & 1, c = e >> (PTC + 4);
+    const int e = t + NT * u;
+    const int j = e & (TC - 1), r = (e >> PTC) & (R - 1), h = (e >> (PTC + LR)) & 1, c = e >> (PTC + LR + 1);
     const int s = h * R + r;
     buf[s * LS + v2_skew((c << PTC) + j)] = Tp[(((c << PA) + slot_k1(s)) << PTC) + j];
   }
   __syncthreads();
-  v2_pass_t<V2_PB, LS, 0, 1, CT>(buf, tw_b);
-  // one slot per thread for all its items: s = t % 16, k2 = t / 16 + 32 u
-  const int s = t & (2 * R - 1), h = s >> 3, r = s & (R - 1), k1 = slot_k1(s);
+  v2_pass_t<V2_PB, LS, 0, 1, CT, NT>(buf, tw_b);
+  // one slot per thread for all its items: s = t % 2R, k2 = t / 2R + KSTEP u
+  constexpr int KSTEP = NT / (2 * R);
+  const int s = t & (2 * R - 1), h = s >> LR, r = s & (R - 1), k1 = slot_k1(s);
   if (MODE == 2) {
     const int keep = nk2_keep < Bc / 2 ? nk2_keep : Bc / 2;
-    for (int q = t >> 4; q < 2 * keep; q += V2_THREADS / 16) {
+    for (int q = t >> (LR + 1); q < 2 * keep; q += KSTEP) {
       const int k2 = q < keep ? q : Bc - 2 * keep + q;          // [0, keep) and [Bc - keep, Bc)
       Zout[lc * Mh + k1 + ((int64_t)k2 << PA)] = buf[s * LS + v2_skew(k2)];
     }
@@ -365,8 +385,8 @@ __device__ __forceinline__ void v2_rows_one(CT* buf, const CT* __restrict__ T, c
   float* prow = fa.power + lcd * fa.F;
   const int64_t jbase = (int64_t)k1 - fa.k0;
   float pmax = 0.0f;
-  constexpr int KSTEP = V2_THREADS / 16, UB = 4;                   // items of a thread: k2 = t / 16 + 32 u
-  for (int k2b = t >> 4; k2b < (int)nK2; k2b += KSTEP * UB) {
+  constexpr int UB = 4;                                            // items of a thread: k2 = t / 2R + KSTEP u
+  for (int k2b = t >> (LR + 1); k2b < (int)nK2; k2b += KSTEP * UB) {
     V2FTab tb[UB];
     int64_t jj[UB];
     bool valid[UB];
@@ -406,16 +426,23 @@ nufft2_rows_kernel(const CT* __restrict__ T, const CT* __restrict__ tw_b, V2Fini
   LKB_DYN_SMEM(CT, buf);
   v2_rows_one<PA, MODE, CT>(buf, T, tw_b, fa, Zout, nk2_keep, (int64_t)blockIdx.y, 0, (int)blockIdx.x);
 }
-// escalation pass (double precision, finish mode): blocks stride over a device-side count of transforms; transform
-// slot lc holds light curve fa.lcmap[nc.base + lc]
-template <int PA>
-__global__ void __launch_bounds__(V2_THREADS, 1)
+// escalation pass (double precision, finish mode, tiles of 2^v2_log_tile(PA, true) points): blocks stride over a
+// device-side count of transforms; transform slot lc holds light curve fa.lcmap[nc.base + lc].  (A call per transform,
+// as in nufft2_cols_list_kernel: no spills.)
+template <int PA, int LOGT>
+__device__ __noinline__ void v2_rows_list_one(double2* buf, const double2* __restrict__ T,
+                                              const double2* __restrict__ tw_b, const V2Finish fa, const int64_t lc,
+                                              const int lc_base) {
+  v2_rows_one<PA, 1, double2, LOGT>(buf, T, tw_b, fa, nullptr, 0, lc, lc_base, (int)blockIdx.x);
+}
+template <int PA, int LOGT = v2_log_tile(PA, true)>
+__global__ void __launch_bounds__((1 << LOGT) / 16, LOGT < V2_LOG_TILE ? 2 : 1)
 nufft2_rows_list_kernel(const double2* __restrict__ T, const double2* __restrict__ tw_b, V2Finish fa, V2Count nc) {
   LKB_DYN_SMEM(double2, buf);
   const int64_t ntr = v2_count(nc, (int)gridDim.y);
   for (int64_t lc = blockIdx.y; lc < ntr; lc += gridDim.y) {
     __syncthreads();
-    v2_rows_one<PA, 1, double2>(buf, T, tw_b, fa, nullptr, 0, lc, nc.base, (int)blockIdx.x);
+    v2_rows_list_one<PA, LOGT>(buf, T, tw_b, fa, lc, nc.base);
   }
 }
 
@@ -447,7 +474,11 @@ __global__ void nufft2_flag_kernel(const unsigned* __restrict__ peak, const floa
   }
 }
 
-// double-precision fine grids of the listed light curves: G[i][e] for light curve list[i0 + i]; grid (cells / 256, n)
+// double-precision fine grids of the listed light curves: G[i][e] for light curve list[nc.base + i], in the layout of
+// the double-precision column kernel (ptc = its log2 columns per CTA).  One thread = one z cell of LCS_D listed light
+// curves, which share the cell's cadence range and kernel weights (the sums of each light curve run in cadence order,
+// as with one light curve per thread); grid (cells / 256, gy), blocks stride over the listed light curves.
+constexpr int LCS_D = 4;
 __global__ void __launch_bounds__(256)
 nufft2_spread_list_kernel(const int32_t* __restrict__ first_ge, const nufft::Cad* __restrict__ cad,
                           const double* __restrict__ Wt, const float* __restrict__ y, int64_t ystride,
@@ -457,28 +488,40 @@ nufft2_spread_list_kernel(const int32_t* __restrict__ first_ge, const nufft::Cad
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= cells) return;
   const int64_t M = (int64_t)1 << p, m = 2 * v2_zcell_of(e, ptc, n1max);
-  const int ntr = v2_count(nc, (int)gridDim.y);
-  for (int i = (int)blockIdx.y; i < ntr; i += (int)gridDim.y) {
-  const float* yr = y + (int64_t)list[nc.base + i] * ystride;
-  double a0 = 0.0, a1 = 0.0;
   const int64_t L = nufft::table_len(M, w);
-  for (int wrap = 0; wrap < 2; ++wrap) {
-    const int64_t mm = m + (int64_t)wrap * M;
-    if (mm + 1 >= L) break;
-    int64_t lo_c = mm - w + 1, hi_c = mm + 2;
-    if (lo_c < 0) lo_c = 0;
-    if (hi_c > L - 1) hi_c = L - 1;
-    const int32_t na = first_ge[lo_c], nb = first_ge[hi_c];
-    for (int32_t n = na; n < nb; ++n) {
-      const int tap = (int)(mm - (int64_t)cad[n].i0);
-      const double* wr = Wt + (int64_t)n * w;
-      const double w0 = (tap >= 0) ? wr[tap] : 0.0, w1 = (tap + 1 < w) ? wr[tap + 1] : 0.0;
-      const double v = (double)yr[n];
-      a0 = fma(w0, v, a0);
-      a1 = fma(w1, v, a1);
+  const int ntr = v2_count(nc, (int)gridDim.y * LCS_D);
+  for (int i0 = (int)blockIdx.y * LCS_D; i0 < ntr; i0 += (int)gridDim.y * LCS_D) {
+    const float* yr[LCS_D];
+#pragma unroll
+    for (int q = 0; q < LCS_D; ++q) {
+      const int i = (i0 + q < ntr) ? i0 + q : ntr - 1;          // clamped slots are computed and dropped
+      yr[q] = y + (int64_t)list[nc.base + i] * ystride;
     }
-  }
-  G[(int64_t)i * cells + e] = make_double2(a0, a1);
+    double a0[LCS_D], a1[LCS_D];
+#pragma unroll
+    for (int q = 0; q < LCS_D; ++q) { a0[q] = 0.0; a1[q] = 0.0; }
+    for (int wrap = 0; wrap < 2; ++wrap) {
+      const int64_t mm = m + (int64_t)wrap * M;
+      if (mm + 1 >= L) break;
+      int64_t lo_c = mm - w + 1, hi_c = mm + 2;
+      if (lo_c < 0) lo_c = 0;
+      if (hi_c > L - 1) hi_c = L - 1;
+      const int32_t na = first_ge[lo_c], nb = first_ge[hi_c];
+      for (int32_t n = na; n < nb; ++n) {
+        const int tap = (int)(mm - (int64_t)cad[n].i0);
+        const double* wr = Wt + (int64_t)n * w;
+        const double w0 = (tap >= 0) ? wr[tap] : 0.0, w1 = (tap + 1 < w) ? wr[tap + 1] : 0.0;
+#pragma unroll
+        for (int q = 0; q < LCS_D; ++q) {
+          const double v = (double)yr[q][n];
+          a0[q] = fma(w0, v, a0[q]);
+          a1[q] = fma(w1, v, a1[q]);
+        }
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < LCS_D; ++q)
+      if (i0 + q < ntr) G[(int64_t)(i0 + q) * cells + e] = make_double2(a0[q], a1[q]);
   }
 }
 
@@ -516,39 +559,34 @@ inline bool v2_supported(int p) { return p >= V2R_P_MIN && p <= V2R_P_MAX; }
 
 template <int PA, class CT>
 int v2_cols_pa(const CT* G, CT* T, int n1max, int B, const V2TablesT<CT>& tb, cudaStream_t st, V2Count nc) {
-  constexpr int A = 1 << PA, TC = V2_TILE / A;
+  constexpr int LOGT = v2_log_tile(PA, sizeof(CT) == 16), A = 1 << PA, TC = (1 << LOGT) / A;
   const size_t smem = (size_t)TC * (A + A / 16 + 1) * sizeof(CT);
   const dim3 grid((unsigned)(V2_BC / TC), (unsigned)B);
-  if constexpr (sizeof(CT) == 16) {
-    if (nc.count) {
-      LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_cols_list_kernel<PA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_cols_list_kernel<PA>)(G, T, n1max, tb.tw_a, tb.t_hi, tb.t_lo, nc);
-      LKB_LAUNCH_CHECK();
-      return LKB_OK;
-    }
+  if constexpr (sizeof(CT) == 16) {          // the escalation pass: always with a device-side count
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_cols_list_kernel<PA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LKB_LAUNCH_SMEM(grid, (1 << LOGT) / 16, smem, st, nufft2_cols_list_kernel<PA>)(G, T, n1max, tb.tw_a, tb.t_hi, tb.t_lo, nc);
+  } else {
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_cols_kernel<PA, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_cols_kernel<PA, CT>)(G, T, n1max, tb.tw_a, tb.t_hi, tb.t_lo);
   }
-  LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_cols_kernel<PA, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_cols_kernel<PA, CT>)(G, T, n1max, tb.tw_a, tb.t_hi, tb.t_lo);
   LKB_LAUNCH_CHECK();
   return LKB_OK;
 }
 template <int PA, class CT>
 int v2_rows_pa(const CT* T, int B, const V2TablesT<CT>& tb, const V2Finish* fa, CT* Zout, int nk2_keep, cudaStream_t st,
                V2Count nc) {
-  const size_t smem = (size_t)(2 * V2_R) * V2_LSB * sizeof(CT);
-  const dim3 grid((unsigned)((1 << PA) / (2 * V2_R)), (unsigned)B);
-  if constexpr (sizeof(CT) == 16) {
-    if (nc.count && fa) {
-      LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_list_kernel<PA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_rows_list_kernel<PA>)(T, tb.tw_b, *fa, nc);
-      LKB_LAUNCH_CHECK();
-      return LKB_OK;
-    }
+  constexpr int LOGT = v2_log_tile(PA, sizeof(CT) == 16), R = (1 << LOGT) / (2 * V2_BC);
+  const size_t smem = (size_t)(2 * R) * V2_LSB * sizeof(CT);
+  const dim3 grid((unsigned)((1 << PA) / (2 * R)), (unsigned)B);
+  if constexpr (sizeof(CT) == 16) {          // the escalation pass: always with a device-side count, finish mode
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_list_kernel<PA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LKB_LAUNCH_SMEM(grid, (1 << LOGT) / 16, smem, st, nufft2_rows_list_kernel<PA>)(T, tb.tw_b, *fa, nc);
+  } else {
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_kernel<PA, 1, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_kernel<PA, 2, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (fa) LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_rows_kernel<PA, 1, CT>)(T, tb.tw_b, *fa, nullptr, 0);
+    else LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_rows_kernel<PA, 2, CT>)(T, tb.tw_b, V2Finish(), Zout, nk2_keep);
   }
-  LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_kernel<PA, 1, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LKB_CUDA_CHECK(cudaFuncSetAttribute(nufft2_rows_kernel<PA, 2, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  if (fa) LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_rows_kernel<PA, 1, CT>)(T, tb.tw_b, *fa, nullptr, 0);
-  else LKB_LAUNCH_SMEM(grid, V2_THREADS, smem, st, nufft2_rows_kernel<PA, 2, CT>)(T, tb.tw_b, V2Finish(), Zout, nk2_keep);
   LKB_LAUNCH_CHECK();
   return LKB_OK;
 }

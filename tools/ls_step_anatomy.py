@@ -4,7 +4,9 @@
 
 Runs the step `--warmup` times, then `--steps` times under torch.profiler with CUDA activities, and sums the device
 time of every kernel by name.  Kernels are grouped into what they do to the flux (prep / spread / low rows /
-escalation / transforms / other), and the card name and power limit are read in the same run.  Writes
+escalation / transforms / other), and the card name and power limit are read in the same run.  Every kernel's launch
+shape (grid, block, dynamic + static shared memory, registers per thread; from the profiler's trace, one entry per
+distinct shape) is recorded beside its time, so that a kernel sized for more work than it has shows as such.  Writes
 DIR/anatomy_<label>.json and prints a table; the JSON holds milliseconds per step.
 """
 import argparse
@@ -12,6 +14,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 from collections import defaultdict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -34,6 +37,26 @@ def group_of(name):
         if any(k in name for k in keys):
             return g
     return "other"
+
+
+def launch_shapes(prof):
+    """kernel name -> distinct launch shapes, read from the profiler's Chrome trace (written to a temporary file)"""
+    shapes = defaultdict(list)
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            events = json.load(f).get("traceEvents", [])
+    for ev in events:
+        if ev.get("cat") != "kernel":
+            continue
+        a = ev.get("args", {})
+        shape = "grid %s block %s smem %s regs %s" % (
+            "x".join(str(v) for v in a.get("grid", [])), "x".join(str(v) for v in a.get("block", [])),
+            a.get("shared memory", "?"), a.get("registers per thread", "?"))
+        if shape not in shapes[ev["name"]]:
+            shapes[ev["name"]].append(shape)
+    return shapes
 
 
 def card_info(torch):
@@ -88,7 +111,9 @@ def main():
         k = per_kernel[ev.name]
         k[0] += ev.device_time / 1000.0           # us -> ms
         k[1] += 1
-    kernels = {name: {"ms_per_step": v[0] / args.steps, "launches_per_step": v[1] / args.steps}
+    shapes = launch_shapes(prof)
+    kernels = {name: {"ms_per_step": v[0] / args.steps, "launches_per_step": v[1] / args.steps,
+                      "launch_shapes": shapes.get(name, [])}
                for name, v in sorted(per_kernel.items(), key=lambda kv: -kv[1][0])}
     groups = defaultdict(float)
     for name, v in kernels.items():
@@ -104,6 +129,8 @@ def main():
     print("%s  %s  %s" % (args.label, rec["card"]["name"], rec["card"]["power_limit_and_max_sm_clock"]))
     for name, v in kernels.items():
         print("  %8.4f ms  x%-5g %-10s %s" % (v["ms_per_step"], v["launches_per_step"], group_of(name), name[:110]))
+        for shape in v["launch_shapes"]:
+            print("  %31s %s" % ("", shape))
     for g, v in sorted(groups.items(), key=lambda kv: -kv[1]):
         print("  group %-10s %8.4f ms" % (g, v))
     print("  kernels total %.4f ms; prep + spread + low rows + escalation %.4f ms" % (rec["kernel_ms_per_step"], replaced))
