@@ -834,7 +834,8 @@ int regress(const double* X, int x_batched, const double* y, const double* flux_
 
 // K8: CBVCorrector.correct_elasticnet (cbvcorrector.py:358-379).  The unit-weight Gram matrix [X | y]^T M [X | y] of
 // the used cadences (K5's first pass, always the exact fp64 kernels: the ~1e-6 relative error of the tcgen05 Gram
-// would move the sweep at which the coordinate descent stops), the coordinate descent (enet.cuh), then the model
+// would move the sweep at which the coordinate descent stops; split over two CTAs by N alone, as under
+// LKB_REGRESS_EXACT_INVARIANT), the coordinate descent (enet.cuh), then the model
 // X[:, :-1] w[:-1] minus its median over all cadences (rg_final on the coefficients with the last one zeroed).
 int elasticnet(const double* X, int x_batched, const double* y, const uint8_t* cadence_mask, int B, int64_t N, int K,
                double alpha, double l1_ratio, int max_iter, double tol, int positive, double* coeff, double* model,
@@ -904,7 +905,9 @@ int elasticnet(const double* X, int x_batched, const double* y, const uint8_t* c
     }
   }
   prof_begin(st);
-  LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, nullptr, B, N, K, 1.0, true, false, ws, st));
+  // exact: the two-CTA split of a light curve depends on N alone, so its Gram matrix (and through the stopping tests
+  // its n_iter and coefficients) does not depend on how many light curves share the call
+  LKB_TRY(rg_gram_pass(d_X, x_batched, d_y, nullptr, B, N, K, 1.0, true, true, ws, st));
   LKB_LAUNCH_CHECK();
   prof_end(st);
   prof_begin(st);
