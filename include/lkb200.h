@@ -314,6 +314,39 @@ int lkb_cdpp(const double* time, const double* flux, const int64_t* offsets, int
              const int32_t* durations, int D, int savgol_window, int savgol_polyorder, double sigma,
              double* cdpp_out, int mem, void* stream);
 
+/* ---- fold and bin (K13) ----------------------------------------------------- */
+/* Replaces LightCurve.fold and LightCurve.bin, lightcurve.py:1089-1214 and 1558-1763, for B light curves at once.
+ * One CTA per light curve; its sort buffers stay in shared memory up to a cap and use a global workspace beyond it.
+ * lkb_fold: rel = ((t - t0) + shift + (period - wrap)) % period - (period - wrap) with numpy's float remainder, then
+ * a stable sort by rel equal to np.argsort(rel, kind="stable") (-0.0 equals +0.0, NaN last).
+ *   time                     [offsets[B]] fp64; offsets int64 [B + 1] HOST memory in both modes
+ *   t0, shift, period, wrap  [B] fp64, HOST memory in both modes; period > 0, else LKB_E_ARG
+ *   normalize                nonzero: the phase is rel / period
+ *   phase_out                [offsets[B]] fp64, the phase in sorted order
+ *   perm_out                 int32 [offsets[B]], the light curve's own cadence index of each sorted position */
+int lkb_fold(const double* time, const int64_t* offsets, int B, const double* t0, const double* shift,
+             const double* period, const double* wrap, int normalize, double* phase_out, int32_t* perm_out,
+             int mem, void* stream);
+/* lkb_bin: the cadences are stably sorted by time; cadence t belongs to bin j = searchsorted(starts, t, "right") - 1
+ * when t < ends[j], or t <= ends[j] in the last bin.  Per bin: the aggregate of the flux (LKB_BIN_NANMEAN: np.nanmean
+ * as a fixed-order sum; LKB_BIN_NANMEDIAN: np.nanmedian), its error (when some flux_err of the light curve is finite:
+ * sqrt(nansum(e^2) / count(isfinite(e))), else the nanstd of the bin's flux), its centre start + 0.5 * (end - start)
+ * and its cadence count.  A bin without a cadence or without a usable value is NaN.
+ *   time, flux, flux_err     [offsets[B]] fp64 (flux_err may be NULL: no errors); offsets HOST memory
+ *   bin_offsets              int64 [B + 1], HOST memory: the CSR of the bins
+ *   starts, ends             [bin_offsets[B]] fp64 edges as times, or NULL ...
+ *   start_idx, end_idx       int32 [bin_offsets[B]] ... edges as indices into the light curve's time-sorted cadences
+ *                            (exactly one of the two pairs is given)
+ *   centre_out, flux_out, err_out  [bin_offsets[B]] fp64; count_out int32 [bin_offsets[B]]
+ * Bin starts that do not ascend (numpy's order, NaN last; for index edges, start indices that decrease) and edge
+ * indices outside [0, n) return LKB_E_ARG naming the light curve.  The call waits for the kernel in both modes. */
+#define LKB_BIN_NANMEAN   0
+#define LKB_BIN_NANMEDIAN 1
+int lkb_bin(const double* time, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+            const int64_t* bin_offsets, const double* starts, const double* ends, const int32_t* start_idx,
+            const int32_t* end_idx, int aggregate, double* centre_out, double* flux_out, double* err_out,
+            int32_t* count_out, int mem, void* stream);
+
 /* ---- batched order statistics (K6) ---------------------------------------- */
 /* nanmedian and nanstd (ddof=0) per light curve: np.nanmedian / np.nanstd as used by
  * normalize (lightcurve.py:1253-1254) and flatten (:1003-1005). out_median/out_std [B]. */

@@ -21,6 +21,7 @@ LS_ALGO_AUTO, LS_ALGO_SIMT, LS_ALGO_TCGEN05, LS_ALGO_NUFFT = 0, 1, 2, 3
 FLATTEN_PATH_V2_MOMENTS, FLATTEN_PATH_V2_DIRECT, FLATTEN_PATH_V1, FLATTEN_PATH_V1_RERUN = 0, 1, 2, 3
 BLS_LIKELIHOOD, BLS_SNR = 0, 1
 REGRESS_EXACT_INVARIANT = 1
+BIN_NANMEAN, BIN_NANMEDIAN = 0, 1
 
 c_int, c_i64, c_dbl, c_vp = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
 
@@ -71,6 +72,9 @@ SIGNATURES = {
     "lkb_nanmedian_std": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp]),
     "lkb_sigma_clip": (c_int, [c_vp, c_vp, c_int, c_dbl, c_dbl, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_cdpp": (c_int, [c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_dbl, c_vp, c_int, c_vp]),
+    "lkb_fold": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp]),
+    "lkb_bin": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+                        c_int, c_vp]),
     "lkb_pg_logmedian": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_dbl, c_vp, c_int, c_vp]),
     "lkb_acf_windows": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_nccl_version": (c_int, []),

@@ -210,6 +210,89 @@ class LightCurveCollection(Collection):
             res = engine.cdpp(times, fluxes, np.asarray(durs, dtype=np.int64), savgol_window, savgol_polyorder, sigma)
         return u.Quantity(res if seq else res[:, 0], u.ppm)
 
+    def fold(self, period=None, epoch_time=None, epoch_phase=0, wrap_phase=None, normalize_phase=False):
+        """Batched ``LightCurve.fold``: equal to ``[lc.fold(...) for lc in collection]``, with the phases of every light
+        curve computed and stably sorted in one GPU call (K13, ``engine.fold``).  `period`, `epoch_time`,
+        `epoch_phase` and `wrap_phase` are each a scalar (float or Quantity) or a sequence of one value per light
+        curve, such as a list of ``pg.period_at_max_power``.  Returns a LightCurveCollection of FoldedLightCurve
+        objects.  The JD warning of `epoch_time` is raised at most once per call."""
+        import warnings
+        from . import engine
+        from .lightcurve import _fold_params
+        from .utils import LightkurveWarning
+        B = len(self.data)
+        if B == 0:
+            return LightCurveCollection([])
+        args = [_per_light_curve(v, B, name) for v, name in ((period, "period"), (epoch_time, "epoch_time"),
+                                                             (epoch_phase, "epoch_phase"), (wrap_phase, "wrap_phase"))]
+        times, params, jd_warning = [], [], None
+        for b, lc in enumerate(self.data):
+            t = np.asarray(lc.time.value, dtype=np.float64)
+            p = _fold_params(t, lc.time, args[0][b], args[1][b], args[2][b], args[3][b], normalize_phase)
+            jd_warning = jd_warning or p[4]
+            times.append(t)
+            params.append(p[:4])
+        if jd_warning:
+            warnings.warn(jd_warning, LightkurveWarning)
+        out = [None] * B
+        batch = [b for b in range(B) if params[b][0] > 0]
+        for b in range(B):
+            if not params[b][0] > 0:                   # numpy's remainder by a zero, negative or NaN period
+                with warnings.catch_warnings():
+                    warnings.simplefilter("ignore", LightkurveWarning)
+                    out[b] = self.data[b].fold(args[0][b], args[1][b], args[2][b], args[3][b], normalize_phase)
+        if batch:
+            per, t0, shift, wrap = (np.array([params[b][k] for b in batch], dtype=np.float64) for k in range(4))
+            res = engine.fold([times[b] for b in batch], t0, shift, per, wrap, normalize=normalize_phase)
+            for k, b in enumerate(batch):
+                out[b] = self.data[b]._folded(times[b], res["perm"][k], res["phase"][k], params[b][0], params[b][1],
+                                              args[1][b], args[2][b], args[3][b], normalize_phase)
+        return LightCurveCollection(out)
+
+    def bin(self, time_bin_size=None, time_bin_start=None, time_bin_end=None, n_bins=None, aggregate_func=None,
+            bins=None, binsize=None):
+        """Batched ``LightCurve.bin``: equal to ``[lc.bin(...) for lc in collection]``, with the same keywords and
+        errors.  With ``aggregate_func`` None, ``np.nanmean`` or ``np.nanmedian``, every light curve is sorted and
+        binned in one GPU call (K13, ``engine.bin``); the nanmean's and the errors' sums then run in a fixed order,
+        so they may differ from the loop's numpy sums in the last bits.  Any other ``aggregate_func`` runs the
+        per-light-curve loop.  Works on folded collections, whose time is the phase.  A zero-length light curve comes
+        back as its copy; a light curve with no bin, or with bin-edge indices that do not ascend, goes through its
+        own single-curve method."""
+        from . import engine
+        from .lightcurve import _bin_check_args, _bin_edges
+        kw = dict(time_bin_size=time_bin_size, time_bin_start=time_bin_start, time_bin_end=time_bin_end,
+                  n_bins=n_bins, aggregate_func=aggregate_func, bins=bins, binsize=binsize)
+        agg = _bin_check_args(time_bin_size, n_bins, aggregate_func, bins, binsize)
+        if agg is np.nanmean or agg is np.nanmedian:
+            aggregate = "nanmean" if agg is np.nanmean else "nanmedian"
+        else:
+            return LightCurveCollection([lc.bin(**kw) for lc in self.data])
+        out = [None] * len(self.data)
+        times = [np.asarray(lc.time.value, dtype=np.float64) for lc in self.data]
+        nonempty = [b for b, t in enumerate(times) if len(t)]
+        for b, t in enumerate(times):
+            if not len(t):
+                out[b] = self.data[b].copy()
+        first, last = _sorted_first_last([times[b] for b in nonempty])
+        batch, starts, ends, kind = [], [], [], None
+        for k, b in enumerate(nonempty):
+            kind, s, e = _bin_edges(len(times[b]), first[k], last[k], time_bin_size, time_bin_start, time_bin_end,
+                                    n_bins, bins, binsize)
+            if len(s) == 0 or not _ascending(s):
+                out[b] = self.data[b].bin(**kw)        # no bin: the single method's IndexError; unordered starts
+                continue
+            batch.append(b)
+            starts.append(s)
+            ends.append(e)
+        if batch:
+            errs = [np.asarray(self.data[b].flux_err.value, dtype=np.float64) for b in batch]
+            res = engine.bin([times[b] for b in batch],
+                             [np.asarray(self.data[b].flux.value, dtype=np.float64) for b in batch], errs, starts,
+                             ends, index_edges=kind == "index", aggregate=aggregate)
+            for k, b in enumerate(batch):
+                out[b] = self.data[b]._binned(res["time"][k], res["flux"][k], res["flux_err"][k])
+        return LightCurveCollection(out)
+
     def stitch(self, corrector_func=lambda x: x.normalize()):
         """Concatenate the light curves (collections.py:196-230)."""
         from .units import Quantity, Time
@@ -222,3 +305,37 @@ class LightCurveCollection(Collection):
         new.flux_err = Quantity(np.concatenate([np.asarray(lc.flux_err.to(first.flux.unit).value) for lc in lcs]),
                                 first.flux.unit)
         return new
+
+
+def _per_light_curve(value, B, name):
+    """`value` repeated for B light curves, or its B elements when it is a sequence or array of one per light curve."""
+    if value is None or isinstance(value, str) or np.ndim(getattr(value, "value", value)) == 0:
+        return [value] * B
+    if len(value) != B:
+        raise ValueError("`{}` has {} values for {} light curves".format(name, len(value), B))
+    return [value[b] for b in range(B)]
+
+
+def _sorted_first_last(times):
+    """First and last value of each array of `times` (all non-empty) once stably sorted in numpy's order (NaN last)."""
+    if not times:
+        return np.zeros(0), np.zeros(0)
+    cat = np.concatenate(times)
+    at = np.cumsum([0] + [len(t) for t in times[:-1]])
+    nan = np.add.reduceat(np.isnan(cat), at)
+    with np.errstate(invalid="ignore"):
+        first = np.fmin.reduceat(cat, at)
+        last = np.where(nan > 0, np.nan, np.fmax.reduceat(cat, at))
+    for b in np.nonzero((first == 0) | (last == 0))[0]:      # which zero, -0.0 or +0.0, comes first / last
+        ts = np.sort(times[b], kind="stable")
+        first[b], last[b] = ts[0], ts[-1]
+    return first, last
+
+
+def _ascending(s):
+    """True when `s` does not decrease in numpy's order (NaN last)."""
+    s = np.asarray(s)
+    if s.dtype.kind != "f":
+        return bool(np.all(s[1:] >= s[:-1]))
+    a, b = s[:-1], s[1:]
+    return not bool(np.any((b < a) | (np.isnan(a) & ~np.isnan(b))))

@@ -238,6 +238,10 @@ int sigma_clip(const double*, const int64_t*, int, double, double, int, uint8_t*
                cudaStream_t);
 int cdpp(const double*, const double*, const int64_t*, int, const int32_t*, int, int, int, double, double*, int,
          cudaStream_t);
+int fold(const double*, const int64_t*, int, const double*, const double*, const double*, const double*, int, double*,
+         int32_t*, int, cudaStream_t);
+int bin(const double*, const double*, const double*, const int64_t*, int, const int64_t*, const double*, const double*,
+        const int32_t*, const int32_t*, int, double*, double*, double*, int32_t*, int, cudaStream_t);
 
 }  // namespace lkb
 
@@ -482,6 +486,22 @@ int lkb_cdpp(const double* time, const double* flux, const int64_t* offsets, int
   std::lock_guard<std::mutex> lk(g_mu);
   return cdpp(time, flux, offsets, B, durations, D, savgol_window, savgol_polyorder, sigma, cdpp_out, mem,
               (cudaStream_t)stream);
+}
+
+int lkb_fold(const double* time, const int64_t* offsets, int B, const double* t0, const double* shift,
+             const double* period, const double* wrap, int normalize, double* phase_out, int32_t* perm_out, int mem,
+             void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return fold(time, offsets, B, t0, shift, period, wrap, normalize, phase_out, perm_out, mem, (cudaStream_t)stream);
+}
+
+int lkb_bin(const double* time, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+            const int64_t* bin_offsets, const double* starts, const double* ends, const int32_t* start_idx,
+            const int32_t* end_idx, int aggregate, double* centre_out, double* flux_out, double* err_out,
+            int32_t* count_out, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return bin(time, flux, flux_err, offsets, B, bin_offsets, starts, ends, start_idx, end_idx, aggregate, centre_out,
+             flux_out, err_out, count_out, mem, (cudaStream_t)stream);
 }
 
 int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_lo, const int32_t* win_hi, int W,

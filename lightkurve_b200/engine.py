@@ -814,6 +814,127 @@ def cdpp(times, fluxes, durations=13, savgol_window=101, savgol_polyorder=2, sig
     return out
 
 
+def _device_csr(x, name, dtype, n=None):
+    """Checks that `x` is a contiguous one-dimensional CUDA tensor of `dtype` (of n values when n is given)."""
+    if not (_is_torch(x) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype == dtype):
+        raise ValueError("device mode: %s must be a contiguous one-dimensional CUDA %s tensor" % (name, dtype))
+    if n is not None and x.numel() != n:
+        raise ValueError("device mode: %s has %d values, the offsets describe %d" % (name, x.numel(), n))
+
+
+def _host_offsets(offsets, what):
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    if off.ndim != 1 or len(off) < 2 or off[0] != 0 or np.any(np.diff(off) < 0):
+        raise ValueError("%s must be a non-decreasing int64 CSR starting at 0" % what)
+    return off
+
+
+def fold(times, t0, shift, period, wrap, normalize=False, offsets=None):
+    """K13.  LightCurve.fold's phase of each light curve, rel = ((t - t0) + shift + (period - wrap)) % period -
+    (period - wrap) (numpy's remainder), stably sorted, divided by the period when `normalize`.  `t0`, `shift`,
+    `period`, `wrap`: one value per light curve (days).  `times`: a list of 1-D arrays (host mode), or the
+    concatenated CUDA float64 tensor with the host int64 CSR `offsets` [B + 1] (device mode, on the current torch
+    stream).  Returns dict(phase, perm): the sorted phases and the int32 permutation (each light curve's own cadence
+    index of each sorted position), as lists of arrays (host) or concatenated tensors (device)."""
+    lib = L.load()
+    if _is_torch(times):
+        import torch
+        if offsets is None:
+            raise ValueError("device mode needs the host CSR `offsets`")
+        off = _host_offsets(offsets, "offsets")
+        _device_csr(times, "times", torch.float64, int(off[-1]))
+        B = len(off) - 1
+    else:
+        B = len(times)
+        if B == 0:
+            return dict(phase=[], perm=[])
+        t, off = _csr(times)
+    pars = [np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (B,))) for v in (t0, shift, period,
+                                                                                                   wrap)]
+    n = int(off[-1])
+    if _is_torch(times):
+        import torch
+        phase = torch.empty(max(n, 1), dtype=torch.float64, device=times.device)
+        perm = torch.empty(max(n, 1), dtype=torch.int32, device=times.device)
+        L.check(lib.lkb_fold(L.ptr(times), L.ptr(off), B, *[L.ptr(p) for p in pars], int(bool(normalize)),
+                             L.ptr(phase), L.ptr(perm), L.MEM_DEVICE, _stream_ptr()))
+        return dict(phase=phase[:n], perm=perm[:n])
+    phase = np.empty(max(n, 1))
+    perm = np.empty(max(n, 1), dtype=np.int32)
+    L.check(lib.lkb_fold(L.ptr(t), L.ptr(off), B, *[L.ptr(p) for p in pars], int(bool(normalize)), L.ptr(phase),
+                         L.ptr(perm), L.MEM_HOST, None))
+    return dict(phase=[phase[off[b]:off[b + 1]] for b in range(B)], perm=[perm[off[b]:off[b + 1]] for b in range(B)])
+
+
+_BIN_AGGREGATES = {"nanmean": L.BIN_NANMEAN, "nanmedian": L.BIN_NANMEDIAN}
+
+
+def bin(times, fluxes, flux_errs, starts, ends, index_edges=False, aggregate="nanmean", offsets=None,
+        bin_offsets=None):
+    """K13.  LightCurve.bin of each light curve with the given bin edges: the cadences are stably sorted by time and
+    cadence t falls in bin j = searchsorted(starts, t, "right") - 1 when t < ends[j] (t <= ends[-1] in the last bin).
+    `starts` / `ends`: per light curve, times (float64) or, with `index_edges`, indices into its time-sorted cadences.
+    `aggregate`: "nanmean" or "nanmedian" of the flux; the error is the root mean square of the finite errors when the
+    light curve has any, else the bin's nanstd of the flux; `flux_errs` may be None (no errors).  Host mode: lists of
+    1-D arrays.  Device mode: concatenated CUDA tensors (float64; int32 index edges) with the host int64 CSRs
+    `offsets` of the cadences and `bin_offsets` of the bins.  Returns dict(time (bin centres), flux, flux_err, count),
+    lists of arrays (host) or concatenated tensors (device)."""
+    lib = L.load()
+    if aggregate not in _BIN_AGGREGATES:
+        raise ValueError("aggregate must be one of %s" % sorted(_BIN_AGGREGATES))
+    agg = _BIN_AGGREGATES[aggregate]
+    if _is_torch(times):
+        import torch
+        if offsets is None or bin_offsets is None:
+            raise ValueError("device mode needs the host CSRs `offsets` and `bin_offsets`")
+        off = _host_offsets(offsets, "offsets")
+        boff = _host_offsets(bin_offsets, "bin_offsets")
+        if len(boff) != len(off):
+            raise ValueError("offsets and bin_offsets describe different numbers of light curves")
+        n, nb = int(off[-1]), int(boff[-1])
+        _device_csr(times, "times", torch.float64, n)
+        _device_csr(fluxes, "fluxes", torch.float64, n)
+        if flux_errs is not None:
+            _device_csr(flux_errs, "flux_errs", torch.float64, n)
+        edt = torch.int32 if index_edges else torch.float64
+        _device_csr(starts, "starts", edt, nb)
+        _device_csr(ends, "ends", edt, nb)
+        B, dev = len(off) - 1, times.device
+        centre, flux, err = (torch.empty(max(nb, 1), dtype=torch.float64, device=dev) for _ in range(3))
+        count = torch.empty(max(nb, 1), dtype=torch.int32, device=dev)
+        e_t = [L.ptr(starts), L.ptr(ends), None, None] if not index_edges else [None, None, L.ptr(starts), L.ptr(ends)]
+        L.check(lib.lkb_bin(L.ptr(times), L.ptr(fluxes), None if flux_errs is None else L.ptr(flux_errs), L.ptr(off),
+                            B, L.ptr(boff), *e_t, agg, L.ptr(centre), L.ptr(flux), L.ptr(err), L.ptr(count),
+                            L.MEM_DEVICE, _stream_ptr()))
+        return dict(time=centre[:nb], flux=flux[:nb], flux_err=err[:nb], count=count[:nb])
+    B = len(times)
+    if B == 0:
+        return dict(time=[], flux=[], flux_err=[], count=[])
+    t, off = _csr(times)
+    f, foff = _csr(fluxes)
+    fe = None
+    if flux_errs is not None:
+        fe, eoff = _csr(flux_errs)
+        if not np.array_equal(off, eoff):
+            raise ValueError("time and flux_err lengths differ")
+    if not np.array_equal(off, foff):
+        raise ValueError("time and flux lengths differ")
+    edt = np.int32 if index_edges else np.float64
+    s, boff = _csr(starts, edt)
+    e, eboff = _csr(ends, edt)
+    if len(boff) != B + 1 or not np.array_equal(boff, eboff):
+        raise ValueError("starts and ends must have one array per light curve, of the same lengths")
+    nb = int(boff[-1])
+    centre, flux, err = np.empty(max(nb, 1)), np.empty(max(nb, 1)), np.empty(max(nb, 1))
+    count = np.empty(max(nb, 1), dtype=np.int32)
+    e_t = [L.ptr(s), L.ptr(e), None, None] if not index_edges else [None, None, L.ptr(s), L.ptr(e)]
+    L.check(lib.lkb_bin(L.ptr(t), L.ptr(f), None if fe is None else L.ptr(fe), L.ptr(off), B, L.ptr(boff), *e_t, agg,
+                        L.ptr(centre), L.ptr(flux), L.ptr(err), L.ptr(count), L.MEM_HOST, None))
+    sl = [slice(boff[b], boff[b + 1]) for b in range(B)]
+    return dict(time=[centre[x] for x in sl], flux=[flux[x] for x in sl], flux_err=[err[x] for x in sl],
+                count=[count[x] for x in sl])
+
+
 def logmedian_windows(frequency, filter_width):
     """Half-open bin ranges of the reference's moving log10-frequency window (periodogram.py:267-277) for an
     ASCENDING frequency grid: window w = { i : |log10 f_i - x0_w| < filter_width }, x0 advancing by

@@ -42,6 +42,89 @@ def _as_flux_quantity(x, unit=None):
     return Quantity(arr, unit, dtype=arr.dtype)
 
 
+def _fold_params(t, time, period, epoch_time, epoch_phase, wrap_phase, normalize_phase):
+    """(period, t0, shift, wrap, JD warning or None) of `LightCurve.fold` in days, for the float64 times `t` of a
+    light curve whose time object is `time`: phase = ((t - t0) + shift + (period - wrap)) % period - (period - wrap).
+    Raises the errors of the single-curve method; the caller issues the warning."""
+    if period is None:
+        raise ValueError("`period` must be given")
+    per = float(np.asarray(Quantity(period, u.day).value)) if u.is_quantity(period) else float(period)
+    t0 = t[0] if epoch_time is None else float(np.asarray(getattr(epoch_time, "value", epoch_time)))
+    jd_warning = None
+    if epoch_time is not None and t0 > 2450000:
+        if time.format == "bkjd":
+            jd_warning = ("`epoch_time` appears to be given in JD, "
+                          "however the light curve time uses BKJD "
+                          "(i.e. JD - 2454833).")
+        elif time.format == "btjd":
+            jd_warning = ("`epoch_time` appears to be given in JD, "
+                          "however the light curve time uses BTJD "
+                          "(i.e. JD - 2457000).")
+    ep = float(np.asarray(getattr(epoch_phase, "value", epoch_phase)))
+    ep_days = ep * per if normalize_phase else (float(np.asarray(Quantity(epoch_phase, u.day).value))
+                                                if u.is_quantity(epoch_phase) else ep)
+    if wrap_phase is None:
+        wrap = per / 2.0
+    else:
+        wv = float(np.asarray(getattr(wrap_phase, "value", wrap_phase)))
+        if normalize_phase:
+            if wv < 0 or wv > 1:
+                raise ValueError("wrap_phase should be between 0 and 1")
+            wrap = wv * per
+        else:
+            wrap = float(np.asarray(Quantity(wrap_phase, u.day).value)) if u.is_quantity(wrap_phase) else wv
+            if wrap < 0 or wrap > per:
+                raise ValueError("wrap_phase should be between 0 and the period")
+    return per, t0, ep_days, wrap, jd_warning
+
+
+def _bin_check_args(time_bin_size, n_bins, aggregate_func, bins, binsize):
+    """Checks the keywords of `LightCurve.bin` as the single-curve method does; returns the aggregate function."""
+    if binsize is not None and bins is not None:
+        raise ValueError("Only one of ``bins`` and ``binsize`` can be specified.")
+    if (binsize is not None or bins is not None) and (time_bin_size is not None or n_bins is not None):
+        raise ValueError("``bins`` or ``binsize`` conflicts with ``n_bins`` or ``time_bin_size``.")
+    if bins is not None:
+        if isinstance(bins, str):
+            if bins in ("blocks", "knuth", "scott", "freedman"):
+                raise NotImplementedError("adaptive ``bins`` rules need astropy.stats, which is not available")
+            raise TypeError("``bins`` must have integer type.")
+        if np.array(bins).dtype.kind not in "iu":
+            raise TypeError("``bins`` must have integer type.")
+    if aggregate_func is None:
+        aggregate_func = np.nanmean
+    if not callable(aggregate_func):
+        raise TypeError("`aggregate_func` must be callable")
+    return aggregate_func
+
+
+def _bin_edges(n, t_first, t_last, time_bin_size, time_bin_start, time_bin_end, n_bins, bins, binsize):
+    """The bin edges of `LightCurve.bin` for a light curve of n > 0 cadences whose stably time-sorted times start with
+    `t_first` and end with `t_last`: ("time", starts, ends) as times, or ("index", starts, ends) as indices into the
+    time-sorted cadences (`binsize` and `bins=<indices>`, whose edges are cadence times)."""
+    as_days = lambda x: float(np.asarray(Quantity(x, u.day).value)) if u.is_quantity(x) else float(x)
+    if binsize is not None:
+        starts = np.arange(n)[::int(binsize)]
+        return "index", starts, np.append(starts[1:], n - 1)
+    if bins is not None and np.size(bins) == 1:
+        edges = np.linspace(t_first, t_last, int(bins) + 1)
+        starts = edges[:-1]
+        return "time", starts, np.append(starts[1:], t_last)
+    if bins is not None:
+        idx = np.asarray(bins, dtype=int)
+        cad = np.arange(n)
+        return "index", cad[idx[:-1]], cad[idx[1:]]
+    size = 0.5 if time_bin_size is None else as_days(time_bin_size)
+    if not size > 0:
+        raise ValueError("`time_bin_size` must be positive")
+    start = t_first if time_bin_start is None else float(getattr(time_bin_start, "value", time_bin_start))
+    if n_bins is None:
+        stop = t_last if time_bin_end is None else float(getattr(time_bin_end, "value", time_bin_end))
+        n_bins = max(1, int(np.ceil((stop - start) / size)))
+    starts = start + size * np.arange(int(n_bins))
+    return "time", starts, starts + size
+
+
 class LightCurve:
     """Time series of flux values (subset of lightkurve.LightCurve).
 
@@ -260,48 +343,17 @@ class LightCurve:
         `binsize` = a new bin every `binsize` cadences, `bins` = a number of equal-width bins or an array of cadence
         indices of the bin edges (astropy's adaptive rules "blocks"/"knuth"/"scott"/"freedman" are not available
         here).  O(N) host code, like the reference's."""
-        if binsize is not None and bins is not None:
-            raise ValueError("Only one of ``bins`` and ``binsize`` can be specified.")
-        if (binsize is not None or bins is not None) and (time_bin_size is not None or n_bins is not None):
-            raise ValueError("``bins`` or ``binsize`` conflicts with ``n_bins`` or ``time_bin_size``.")
-        if bins is not None:
-            if isinstance(bins, str):
-                if bins in ("blocks", "knuth", "scott", "freedman"):
-                    raise NotImplementedError("adaptive ``bins`` rules need astropy.stats, which is not available")
-                raise TypeError("``bins`` must have integer type.")
-            if np.array(bins).dtype.kind not in "iu":
-                raise TypeError("``bins`` must have integer type.")
-        if aggregate_func is None:
-            aggregate_func = np.nanmean
-        if not callable(aggregate_func):
-            raise TypeError("`aggregate_func` must be callable")
+        aggregate_func = _bin_check_args(time_bin_size, n_bins, aggregate_func, bins, binsize)
         order = np.argsort(np.asarray(self.time.value, dtype=np.float64), kind="stable")
         t = np.asarray(self.time.value, dtype=np.float64)[order]
         f = np.asarray(self.flux.value, dtype=np.float64)[order]
         fe = np.asarray(self.flux_err.value, dtype=np.float64)[order]
         if len(t) == 0:
             return self.copy()
-        as_days = lambda x: float(np.asarray(Quantity(x, u.day).value)) if u.is_quantity(x) else float(x)
-        if binsize is not None:
-            starts = t[::int(binsize)]
-            ends = np.append(starts[1:], t[-1])
-        elif bins is not None and np.size(bins) == 1:
-            edges = np.linspace(t[0], t[-1], int(bins) + 1)
-            starts = edges[:-1]
-            ends = np.append(starts[1:], t[-1])
-        elif bins is not None:
-            idx = np.asarray(bins, dtype=int)
-            starts, ends = t[idx[:-1]], t[idx[1:]]
-        else:
-            size = 0.5 if time_bin_size is None else as_days(time_bin_size)
-            if not size > 0:
-                raise ValueError("`time_bin_size` must be positive")
-            start = t[0] if time_bin_start is None else float(getattr(time_bin_start, "value", time_bin_start))
-            if n_bins is None:
-                stop = t[-1] if time_bin_end is None else float(getattr(time_bin_end, "value", time_bin_end))
-                n_bins = max(1, int(np.ceil((stop - start) / size)))
-            starts = start + size * np.arange(int(n_bins))
-            ends = starts + size
+        kind, starts, ends = _bin_edges(len(t), t[0], t[-1], time_bin_size, time_bin_start, time_bin_end, n_bins,
+                                        bins, binsize)
+        if kind == "index":
+            starts, ends = t[starts], t[ends]
         nb = len(starts)
         which = np.searchsorted(starts, t, side="right") - 1                  # last bin starting at or before t
         inside = (which >= 0) & ((t < ends[np.clip(which, 0, nb - 1)]) | ((which == nb - 1) & (t <= ends[-1])))
@@ -319,10 +371,13 @@ class LightCurve:
                 else:
                     v = f[sel]
                     berr[j] = np.nanstd(v) if np.any(np.isfinite(v)) else np.nan
+        return self._binned(starts + 0.5 * (ends - starts), bflux, berr)
+
+    def _binned(self, centres, bflux, berr):
+        """The light curve of bin centres, aggregated flux and errors that `bin` returns."""
         new = self.__class__.__new__(self.__class__)
         new.meta = _copy.deepcopy(self.meta)
         new._columns = {}
-        centres = starts + 0.5 * (ends - starts)
         if isinstance(self.time, Time):
             new.time = Time(centres, self.time.format, self.time.scale)
         else:                                                   # a folded light curve: "time" is the phase
@@ -501,40 +556,20 @@ class LightCurve:
         """Returns a `FoldedLightCurve` folded on a period and epoch (lightcurve.py:1089-1214, which wraps
         astropy TimeSeries.fold): phase = ((t - epoch_time) + epoch_phase + (P - wrap)) % P - (P - wrap),
         sorted by phase; a bare float period / epoch_phase is in days."""
-        if period is None:
-            raise ValueError("`period` must be given")
-        per = float(np.asarray(Quantity(period, u.day).value)) if u.is_quantity(period) else float(period)
         t = np.asarray(self.time.value, dtype=np.float64)
-        t0 = t[0] if epoch_time is None else float(np.asarray(getattr(epoch_time, "value", epoch_time)))
-        if epoch_time is not None and t0 > 2450000:
-            if self.time.format == "bkjd":
-                warnings.warn("`epoch_time` appears to be given in JD, "
-                              "however the light curve time uses BKJD "
-                              "(i.e. JD - 2454833).", LightkurveWarning)
-            elif self.time.format == "btjd":
-                warnings.warn("`epoch_time` appears to be given in JD, "
-                              "however the light curve time uses BTJD "
-                              "(i.e. JD - 2457000).", LightkurveWarning)
-        ep = float(np.asarray(getattr(epoch_phase, "value", epoch_phase)))
-        ep_days = ep * per if normalize_phase else (float(np.asarray(Quantity(epoch_phase, u.day).value))
-                                                    if u.is_quantity(epoch_phase) else ep)
-        if wrap_phase is None:
-            wrap = per / 2.0
-        else:
-            wv = float(np.asarray(getattr(wrap_phase, "value", wrap_phase)))
-            if normalize_phase:
-                if wv < 0 or wv > 1:
-                    raise ValueError("wrap_phase should be between 0 and 1")
-                wrap = wv * per
-            else:
-                wrap = float(np.asarray(Quantity(wrap_phase, u.day).value)) if u.is_quantity(wrap_phase) else wv
-                if wrap < 0 or wrap > per:
-                    raise ValueError("wrap_phase should be between 0 and the period")
-        rel = ((t - t0) + ep_days + (per - wrap)) % per - (per - wrap)
+        per, t0, shift, wrap, jd_warning = _fold_params(t, self.time, period, epoch_time, epoch_phase, wrap_phase,
+                                                        normalize_phase)
+        if jd_warning:
+            warnings.warn(jd_warning, LightkurveWarning)
+        rel = ((t - t0) + shift + (per - wrap)) % per - (per - wrap)
         order = np.argsort(rel, kind="stable")
+        phase = rel[order] / per if normalize_phase else rel[order]
+        return self._folded(t, order, phase, per, t0, epoch_time, epoch_phase, wrap_phase, normalize_phase)
+
+    def _folded(self, t, order, phase, per, t0, epoch_time, epoch_phase, wrap_phase, normalize_phase):
+        """The `FoldedLightCurve` of the cadences in `order` at the sorted `phase` that `fold` returns."""
         folded = FoldedLightCurve.__new__(FoldedLightCurve)
         folded.meta = _copy.deepcopy(self.meta)
-        phase = rel[order] / per if normalize_phase else rel[order]
         folded.time = Quantity(phase, u.dimensionless_unscaled if normalize_phase else u.day)
         folded.flux = Quantity(np.asarray(self.flux.value)[order], self.flux.unit, dtype=self.flux.dtype)
         folded.flux_err = Quantity(np.asarray(self.flux_err.value)[order], self.flux_err.unit, dtype=self.flux_err.dtype)
