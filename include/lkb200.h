@@ -221,6 +221,52 @@ int lkb_bls_stats(const double* t, const double* y, const double* dy, const int6
                   int32_t* per_transit_count, double* per_transit_ll, uint8_t* in_transit, int32_t* status,
                   int mem, void* stream);
 
+/* K14: the steps between the rounds of an iterative search for several transiting planets per light curve
+ * (LightCurveCollection.find_transit_candidates: search, take the best candidate, remove its transits, search again).
+ *
+ * lkb_bls_best: np.nanargmax of each light curve's K3 power and the K3 outputs there - BoxLeastSquaresPeriodogram's
+ * period_at_max_power, duration_at_max_power, transit_time_at_max_power, depth_at_max_power ... for B periodograms.
+ *   power, depth, depth_err, duration, transit_time, depth_snr   K3 outputs (lkb_bls_power_ex), same layout
+ *   period          the K3 grid: period_offsets == NULL: one grid [P] shared by all light curves, outputs [B,P];
+ *                   else a HOST CSR int64 [B+1] into period and the outputs (no light curve with an empty segment)
+ *   *_out           [B] fp64: period_out is 1 / (1 / period[k]) (the periodogram's frequency axis is 1 / period),
+ *                   the others the K3 outputs at k; NaN where every power of the light curve is NaN
+ *   index_out       [B] int64: k, the first index of the largest non-NaN power of the segment; -1 if all are NaN
+ * One CTA per light curve; the winner does not depend on the reduction order.
+ *
+ * lkb_transit_compact: lc[~get_transit_mask(P, D, T0)] of every light curve, from the in_transit flags and the stats of
+ * one lkb_bls_stats call on the same cadences: with fewer than half the cadences in transit the removed cadences are
+ * the in-transit ones, with more the out-of-transit ones, with exactly half those whose level differs from the mean
+ * of the two levels (get_transit_mask_batch's rule; a box that covers every cadence removes nothing).  The survivors
+ * keep their order.
+ *   t, y, dy        [offsets[B]] fp64 times, fluxes and flux errors (any values, NaN included) of this round
+ *   index           [offsets[B]] int32: each cadence's position in its original light curve
+ *   offsets         HOST CSR int64 [B+1]
+ *   in_transit      [offsets[B]] uint8 and stats [B, LKB_BLS_STATS_NCOL]: lkb_bls_stats' outputs
+ *   round           0 .. 127, written into masked_in at the original position of every removed cadence
+ *   orig_offsets    HOST CSR int64 [B+1] of the original light curves (each at least as long as this round's)
+ *   masked_in       int8 [orig_offsets[B]], read and written
+ *   t_out, y_out, dy_out, index_out  the survivors (allocate offsets[B] values; offsets_out[B] are written)
+ *   w_out           the weights of the next search: dy where every surviving dy of the light curve is finite, else 1
+ *                   (BoxLeastSquaresPeriodogram's choice between flux_err and unit weights)
+ *   offsets_out     HOST int64 [B+1] out: CSR of the survivors
+ *   step_offsets_out HOST int64 [B+1] out: CSR of steps, max(n_b - 1, 0) values per light curve
+ *   time_info       [B, 3] fp64: first, smallest and largest surviving time (NaN without survivors)
+ *   dy_finite       [B] uint8: 1 when every surviving dy is finite
+ *   steps           fp64 (allocate offsets[B] values): np.diff of each light curve's surviving times, for
+ *                   lkb_nanmedian_std (the median time step of the next period grid)
+ * The call synchronises once, after counting the survivors, to build offsets_out.  Errors name the light curve. */
+int lkb_bls_best(const double* power, const double* depth, const double* depth_err, const double* duration,
+                 const double* transit_time, const double* depth_snr, const double* period,
+                 const int64_t* period_offsets, int B, int64_t P, double* period_out, double* duration_out,
+                 double* transit_time_out, double* depth_out, double* depth_err_out, double* depth_snr_out,
+                 double* power_out, int64_t* index_out, int mem, void* stream);
+int lkb_transit_compact(const double* t, const double* y, const double* dy, const int32_t* index,
+                        const int64_t* offsets, int B, const uint8_t* in_transit, const double* stats, int round,
+                        const int64_t* orig_offsets, int8_t* masked_in, double* t_out, double* y_out, double* dy_out,
+                        double* w_out, int32_t* index_out, int64_t* offsets_out, int64_t* step_offsets_out,
+                        double* time_info, uint8_t* dy_finite, double* steps, int mem, void* stream);
+
 /* Debug/parity entry: the per-sample bin index of bls.c for ONE period,
  * ind[n] = (int)(fabs(fmod(t[n]-min_t, period))/bin_duration)+1, evaluated by the
  * same device function the search kernel uses. */

@@ -57,6 +57,10 @@ SIGNATURES = {
     "lkb_bls_bin_index": (c_int, [c_vp, c_i64, c_dbl, c_dbl, c_dbl, c_vp, c_int, c_vp]),
     "lkb_bls_stats": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                               c_vp, c_vp, c_int, c_vp]),
+    "lkb_bls_best": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp,
+                             c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
+    "lkb_transit_compact": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+                                    c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_flatten": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_dbl, c_int, c_dbl,
                             c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_flatten_last_path": (c_int, []),

@@ -121,6 +121,64 @@ class LightCurveCollection(Collection):
                                                           None if norm != "psd" else scales, p0["ls_method"])
         return [LombScarglePeriodogram._finish(p, powers[b]) for b, p in enumerate(preps)]
 
+    def find_transit_candidates(self, n_candidates=3, return_stats=False, **kwargs):
+        """Search every light curve for `n_candidates` transiting planets, one after the other, in one GPU call (K3,
+        K14, K10, K6; ``engine.bls_find_candidates``).  For each light curve it equals this loop, from
+        ``lc = lc.remove_nans()``, repeated `n_candidates` times::
+
+            pg = lc.to_periodogram("bls", **kwargs)
+            P, D, T0 = pg.period_at_max_power, pg.duration_at_max_power, pg.transit_time_at_max_power
+            # record P, D, T0 and the depth, depth error, depth_snr and power at max power
+            lc = lc[~pg.get_transit_mask(period=P, duration=D, transit_time=T0)]
+
+        `kwargs` are those of ``to_periodogram("bls")`` (duration, period, minimum_period, maximum_period,
+        frequency_factor, time_unit, objective, oversample) and apply in every round; without `period` each round's
+        grid follows from the survivors of the round before.  Every light curve gets `n_candidates` rounds; filter on
+        ``depth_snr`` to keep the significant ones.  A box that covers every cadence removes none, so the next round
+        finds it again, as the loop does.
+
+        Returns a dict: "period", "duration", "transit_time", "depth", "depth_err", "depth_snr", "power", float64
+        arrays [B, n_candidates] in each light curve's units (time_unit for period and duration, its time format for
+        transit_time, its flux unit for the depths); "masked_in", one int8 array per ``lc.remove_nans()``: the round
+        whose mask removed the cadence, -1 if none, so that ``lc.remove_nans()[masked_in[b] == -1]`` is the loop's
+        last light curve; with `return_stats`, "stats": for each light curve a list of the `n_candidates` dicts of
+        ``pg.compute_stats(P, D, T0)`` (equal to the loop's to the rounding of ``compute_stats_batch``).
+
+        Errors are those of the loop, of the same type, for the first light curve and round at which the loop would
+        raise, naming both.  Times must be finite.  At most 65 535 light curves."""
+        from types import SimpleNamespace
+        from . import engine
+        from .periodogram import BoxLeastSquaresPeriodogram as BLS
+        n_candidates = int(n_candidates)
+        if not 1 <= n_candidates <= 127:
+            raise ValueError("n_candidates must be in 1 .. 127, got {}".format(n_candidates))
+        lcs = [lc.remove_nans() for lc in self.data]
+        B = len(lcs)
+        if B == 0:
+            out = {k: np.zeros((0, n_candidates)) for k in engine.BLS_CANDIDATE_FIELDS}
+            out["masked_in"] = []
+            if return_stats:
+                out["stats"] = []
+            return out
+        times = [np.asarray(lc.time.value, dtype=np.float64) for lc in lcs]
+        for b, t in enumerate(times):
+            if not np.isfinite(t).all():
+                raise ValueError("light curve {} has non-finite times".format(b))
+        shared = kwargs.get("period", None) is not None
+
+        def grid(b, r, tmin, tmax, median_dt):
+            return BLS._grid(tmin, tmax, median_dt, **dict(kwargs))
+
+        res = engine.bls_find_candidates(times, [np.asarray(lc.flux.value, dtype=np.float64) for lc in lcs],
+                                         [np.asarray(lc.flux_err.value, dtype=np.float64) for lc in lcs], grid,
+                                         n_candidates, shared_grid=shared, return_stats=return_stats)
+        if return_stats:
+            owners = [SimpleNamespace(flux=lc.flux, time=lc.time) for lc in lcs]
+            res["stats"] = [[BLS._k10_stats_dict(owners[b], rs["tstart"][b], res["period"][b, r],
+                                                 res["transit_time"][b, r], rs, b)
+                             for r, rs in enumerate(res["stats"])] for b in range(B)]
+        return res
+
     def flatten(self, window_length=101, polyorder=2, return_trend=False, break_tolerance=5, niters=3, sigma=3,
                 mask=None):
         """Batched ``LightCurve.flatten``; `mask` is None or a list of per-LC boolean masks."""

@@ -242,6 +242,12 @@ int fold(const double*, const int64_t*, int, const double*, const double*, const
          int32_t*, int, cudaStream_t);
 int bin(const double*, const double*, const double*, const int64_t*, int, const int64_t*, const double*, const double*,
         const int32_t*, const int32_t*, int, double*, double*, double*, int32_t*, int, cudaStream_t);
+int bls_best(const double*, const double*, const double*, const double*, const double*, const double*, const double*,
+             const int64_t*, int, int64_t, double*, double*, double*, double*, double*, double*, double*, int64_t*, int,
+             cudaStream_t);
+int transit_compact(const double*, const double*, const double*, const int32_t*, const int64_t*, int, const uint8_t*,
+                    const double*, int, const int64_t*, int8_t*, double*, double*, double*, double*, int32_t*,
+                    int64_t*, int64_t*, double*, uint8_t*, double*, int, cudaStream_t);
 
 }  // namespace lkb
 
@@ -502,6 +508,28 @@ int lkb_bin(const double* time, const double* flux, const double* flux_err, cons
   std::lock_guard<std::mutex> lk(g_mu);
   return bin(time, flux, flux_err, offsets, B, bin_offsets, starts, ends, start_idx, end_idx, aggregate, centre_out,
              flux_out, err_out, count_out, mem, (cudaStream_t)stream);
+}
+
+int lkb_bls_best(const double* power, const double* depth, const double* depth_err, const double* duration,
+                 const double* transit_time, const double* depth_snr, const double* period,
+                 const int64_t* period_offsets, int B, int64_t P, double* period_out, double* duration_out,
+                 double* transit_time_out, double* depth_out, double* depth_err_out, double* depth_snr_out,
+                 double* power_out, int64_t* index_out, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return bls_best(power, depth, depth_err, duration, transit_time, depth_snr, period, period_offsets, B, P, period_out,
+                  duration_out, transit_time_out, depth_out, depth_err_out, depth_snr_out, power_out, index_out, mem,
+                  (cudaStream_t)stream);
+}
+
+int lkb_transit_compact(const double* t, const double* y, const double* dy, const int32_t* index,
+                        const int64_t* offsets, int B, const uint8_t* in_transit, const double* stats, int round,
+                        const int64_t* orig_offsets, int8_t* masked_in, double* t_out, double* y_out, double* dy_out,
+                        double* w_out, int32_t* index_out, int64_t* offsets_out, int64_t* step_offsets_out,
+                        double* time_info, uint8_t* dy_finite, double* steps, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return transit_compact(t, y, dy, index, offsets, B, in_transit, stats, round, orig_offsets, masked_in, t_out, y_out,
+                         dy_out, w_out, index_out, offsets_out, step_offsets_out, time_info, dy_finite, steps, mem,
+                         (cudaStream_t)stream);
 }
 
 int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_lo, const int32_t* win_hi, int W,

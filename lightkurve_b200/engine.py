@@ -463,6 +463,179 @@ def _bls_stats_device(lib, t, y, dy, period, duration, transit_time, return_mask
     return res
 
 
+BLS_CANDIDATE_FIELDS = ("period", "duration", "transit_time", "depth", "depth_err", "depth_snr", "power")
+
+
+def _named_error(e, b, r):
+    """`e` again, of the same type, with the light curve and round in front of its message."""
+    try:
+        return type(e)("light curve %d, round %d: %s" % (b, r, e))
+    except Exception:                                  # an exception type that needs other arguments
+        return e
+
+
+def bls_find_candidates(times, fluxes, flux_errs, grid, n_candidates, shared_grid=False, return_stats=False):
+    """K3 + K14 + K10 + K6.  `n_candidates` rounds of search, take the best candidate, remove its transits, for every
+    light curve at once, with the cadences on the device throughout:
+      1. lkb_bls_power_ex on each light curve's survivors (round 0: all its cadences), weights flux_err where every
+         surviving flux_err is finite, else unit weights;
+      2. lkb_bls_best: the candidate at np.nanargmax of the power;
+      3. lkb_bls_stats at the candidate: in-transit flags and box levels (and, with return_stats, its statistics);
+      4. lkb_transit_compact: lc[~get_transit_mask] and what the next grid needs;
+      5. lkb_nanmedian_std of the survivors' time steps.
+    `times`, `fluxes`, `flux_errs`: lists of host arrays (finite times; any flux_err).  `grid(b, r, tmin, tmax,
+    median_dt)` returns dict(period, duration, oversample, objective) for light curve b in round r from its survivors'
+    time span (tmin / tmax None without survivors) and np.median(np.diff(t)) - or raises as the single-curve loop would;
+    duration, oversample and objective must be the same for all.  With `shared_grid` every call returns the same
+    period grid and K3 runs its shared-grid entry.
+    Returns dict of [B, n_candidates] float64 arrays (BLS_CANDIDATE_FIELDS), "masked_in" (list of B int8 arrays: the
+    round that removed each cadence, -1 if none) and, with return_stats, "stats": per round, a host-mode-style
+    bls_stats result (plus "tstart", each light curve's first surviving time).  The first error in the order of the
+    single-curve loop (light curve by light curve, round by round) is raised with its type, naming both."""
+    import torch
+    lib = L.load()
+    B = len(times)
+    if not 0 < B <= 65535:
+        raise ValueError("bls_find_candidates needs 1 .. 65535 light curves, got %d" % B)
+    if not 1 <= int(n_candidates) <= 127:
+        raise ValueError("n_candidates must be in 1 .. 127, got %r" % (n_candidates,))
+    n_candidates = int(n_candidates)
+    t_h, off0 = _csr(times)
+    y_h, _ = _csr(fluxes)
+    dy_h, _ = _csr(flux_errs)
+    if len(y_h) != len(t_h) or len(dy_h) != len(t_h):
+        raise ValueError("time, flux and flux_err lengths differ")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    f64 = dict(dtype=torch.float64, device=dev)
+    n_h = np.diff(off0)
+    # round 0's grid inputs straight from the host arrays (numpy's own reductions)
+    tinfo = np.full((B, 3), np.nan)
+    med = np.full(B, np.nan)
+    w_h = dy_h.copy()
+    for b in range(B):
+        tb = t_h[off0[b]:off0[b + 1]]
+        if len(tb):
+            tinfo[b] = tb[0], np.min(tb), np.max(tb)
+        if len(tb) > 1:
+            med[b] = np.median(np.diff(tb))
+        if not np.isfinite(dy_h[off0[b]:off0[b + 1]]).all():
+            w_h[off0[b]:off0[b + 1]] = 1.0
+
+    def up(a, dtype=torch.float64):
+        x = torch.empty(max(len(a), 1), dtype=dtype, device=dev)
+        x[:len(a)].copy_(torch.from_numpy(np.ascontiguousarray(a)))
+        return x
+
+    d_t, d_y, d_dy, d_w = up(t_h), up(y_h), up(dy_h), up(w_h)
+    d_idx = up(np.concatenate([np.arange(n, dtype=np.int32) for n in n_h]) if len(t_h) else np.zeros(0, np.int32),
+               torch.int32)
+    masked = torch.full((max(int(off0[-1]), 1),), -1, dtype=torch.int8, device=dev)
+    off = off0.copy()
+    out = {k: np.full((B, n_candidates), np.nan) for k in BLS_CANDIDATE_FIELDS}
+    rounds_stats = []
+    err = None                                         # (b, r, exception): the loop's first error so far
+    Bc = B                                             # light curves still searched: those before the first error
+    dur_t = None
+    for r in range(n_candidates):
+        # 1. the grids, on the host; an error truncates the batch to the light curves before it
+        grids = []
+        for b in range(Bc):
+            try:
+                g = grid(b, r, None if n_h[b] == 0 else np.float64(tinfo[b, 1]),
+                         None if n_h[b] == 0 else np.float64(tinfo[b, 2]), np.float64(med[b]))
+            except Exception as e:                     # noqa: BLE001 - whatever the loop raises is raised
+                err, Bc = (b, r, e), b
+                break
+            grids.append(g)
+        if Bc == 0:
+            break
+        g0 = grids[0]
+        if dur_t is None:
+            duration = np.ascontiguousarray(g0["duration"], dtype=np.float64)
+            dur_t = up(duration)
+            oversample, objective = int(g0["oversample"]), (L.BLS_SNR if g0["objective"] == "snr" else L.BLS_LIKELIHOOD)
+        if shared_grid:
+            per_h, pofs = np.ascontiguousarray(g0["period"], dtype=np.float64), None
+            P = len(per_h)
+            total_p = Bc * P
+        else:
+            per_h, pofs = _csr([g["period"] for g in grids])
+            P = int(pofs[-1])
+            total_p = P
+        d_per = up(per_h)
+        k3 = [torch.empty(total_p, **f64) for _ in range(7)]
+        o = np.ascontiguousarray(off[:Bc + 1])
+        L.check(lib.lkb_bls_power_ex(L.ptr(d_t), L.ptr(d_y), L.ptr(d_w), L.ptr(o), Bc, L.ptr(d_per), L.ptr(pofs), P,
+                                     L.ptr(dur_t), len(duration), oversample, objective,
+                                     *[L.ptr(x) for x in k3], None, L.MEM_DEVICE, _stream_ptr()))
+        # 2. the candidates
+        cand = torch.empty((7, Bc), **f64)
+        idx = torch.empty(Bc, dtype=torch.int64, device=dev)
+        L.check(lib.lkb_bls_best(*[L.ptr(x) for x in k3[:6]], L.ptr(d_per), L.ptr(pofs), Bc, P,
+                                 *[L.ptr(cand[k]) for k in range(7)], L.ptr(idx), L.MEM_DEVICE, _stream_ptr()))
+        del k3
+        cand_h, idx_h = cand.cpu().numpy(), idx.cpu().numpy()
+        nan_lc = np.flatnonzero(idx_h < 0)
+        if len(nan_lc):
+            err, Bc = (int(nan_lc[0]), r, ValueError("All-NaN slice encountered")), int(nan_lc[0])
+            if Bc == 0:
+                break
+        for k, name in enumerate(BLS_CANDIDATE_FIELDS):
+            out[name][:Bc, r] = cand_h[k, :Bc]
+        # 3. in-transit flags and levels (and the statistics) at the candidates
+        per_c, dur_c, tt_c = cand_h[0, :Bc], cand_h[1, :Bc], cand_h[2, :Bc]
+        t0 = tinfo[:Bc, 0]
+        ttr = tt_c - t0
+        caps = np.rint((tinfo[:Bc, 2] - t0 - ttr) / per_c) - np.rint((tinfo[:Bc, 1] - t0 - ttr) / per_c) + 1
+        toff = np.zeros(Bc + 1, np.int64)
+        np.cumsum(caps.astype(np.int64), out=toff[1:])
+        o = np.ascontiguousarray(off[:Bc + 1])
+        n_now = int(o[-1])
+        st = _bls_stats_device(lib, d_t[:n_now], d_y[:n_now], d_w[:n_now], cand[0, :Bc].contiguous(),
+                               cand[1, :Bc].contiguous(), cand[2, :Bc].contiguous(), True, o, toff)
+        if return_stats:
+            sh = {k: (v.cpu().numpy() if torch.is_tensor(v) else v) for k, v in st.items() if k != "in_transit"}
+            sh["tstart"] = t0.copy()
+            bad = np.flatnonzero(sh["status"] == L.E_SINGULAR)
+            if len(bad):
+                err, Bc = (int(bad[0]), r, np.linalg.LinAlgError("Singular matrix")), int(bad[0])
+                if Bc == 0:
+                    break
+                o = np.ascontiguousarray(off[:Bc + 1])
+                n_now = int(o[-1])
+            rounds_stats.append(sh)
+        # 4. lc[~mask], with what the next round's grid needs
+        nt, ny, ndy, nw = (torch.empty(max(n_now, 1), **f64) for _ in range(4))
+        nidx = torch.empty(max(n_now, 1), dtype=torch.int32, device=dev)
+        steps = torch.empty(max(n_now, 1), **f64)
+        ti = torch.empty((Bc, 3), **f64)
+        fin = torch.empty(Bc, dtype=torch.uint8, device=dev)
+        noff, soff = np.zeros(Bc + 1, np.int64), np.zeros(Bc + 1, np.int64)
+        L.check(lib.lkb_transit_compact(L.ptr(d_t), L.ptr(d_y), L.ptr(d_dy), L.ptr(d_idx), L.ptr(o), Bc,
+                                        L.ptr(st["in_transit"]), L.ptr(st["stats"][:Bc]), r,
+                                        L.ptr(np.ascontiguousarray(off0[:Bc + 1])), L.ptr(masked), L.ptr(nt),
+                                        L.ptr(ny), L.ptr(ndy), L.ptr(nw), L.ptr(nidx), L.ptr(noff), L.ptr(soff),
+                                        L.ptr(ti), L.ptr(fin), L.ptr(steps), L.MEM_DEVICE, _stream_ptr()))
+        d_t, d_y, d_dy, d_w, d_idx = nt, ny, ndy, nw, nidx
+        off = noff
+        n_h = np.diff(off)
+        # 5. the median time step of the survivors
+        if r + 1 < n_candidates:
+            md = torch.empty(Bc, **f64)
+            L.check(lib.lkb_nanmedian_std(L.ptr(steps), L.ptr(soff), Bc, L.ptr(md), None, L.MEM_DEVICE,
+                                          _stream_ptr()))
+            tinfo[:Bc] = ti.cpu().numpy()
+            med[:Bc] = md.cpu().numpy()
+    if err is not None:
+        b, r, e = err
+        raise _named_error(e, b, r) from e
+    m = masked.cpu().numpy()
+    out["masked_in"] = [m[off0[b]:off0[b + 1]].copy() for b in range(B)]
+    if return_stats:
+        out["stats"] = rounds_stats
+    return out
+
+
 def bls_bin_index(t_rel, min_t, period, bin_duration):
     lib = L.load()
     t_rel = np.ascontiguousarray(t_rel, dtype=np.float64)

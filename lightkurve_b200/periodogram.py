@@ -465,8 +465,14 @@ class BoxLeastSquaresPeriodogram(Periodogram):
                    frequency_factor=1.0):
         """astropy BoxLeastSquares.autoperiod (closed form; called at periodogram.py:1163-1168)."""
         t = np.asarray(time, dtype=np.float64)
+        return BoxLeastSquaresPeriodogram._autoperiod_baseline(t.max() - t.min(), duration, minimum_period,
+                                                               maximum_period, minimum_n_transit, frequency_factor)
+
+    @staticmethod
+    def _autoperiod_baseline(baseline, duration, minimum_period=None, maximum_period=None, minimum_n_transit=3,
+                             frequency_factor=1.0):
+        """autoperiod of light curves whose times span `baseline` (max t - min t): the grid depends on nothing else."""
         duration = np.atleast_1d(np.asarray(duration, dtype=np.float64))
-        baseline = t.max() - t.min()
         df = frequency_factor * duration.min() / baseline ** 2
         if minimum_period is None:
             minimum_period = 2.0 * duration.max()
@@ -489,6 +495,21 @@ class BoxLeastSquaresPeriodogram(Periodogram):
         lc = lc.remove_nans()
         flux_err = np.asarray(lc.flux_err.value, dtype=np.float64)
         dy = flux_err if np.isfinite(flux_err).all() else None
+        tval = np.asarray(lc.time.value, dtype=np.float64)
+        tmin, tmax = (np.min(tval), np.max(tval)) if len(tval) else (None, None)
+        grid = BoxLeastSquaresPeriodogram._grid(tmin, tmax, lambda: np.median(np.diff(tval)), **kwargs)
+        return dict(lc=lc, time=tval, flux=np.asarray(lc.flux.value, dtype=np.float64), dy=dy, **grid)
+
+    @staticmethod
+    def _grid(tmin, tmax, median_dt, **kwargs):
+        """The keyword handling, warnings, errors and period grid of _prepare for a light curve whose times (NaN flux
+        removed) span tmin .. tmax; None for both when it has no cadence, which raises numpy's error where _prepare
+        first reduces its times.  `median_dt`: np.median(np.diff(times)), or a function returning it, asked for only
+        when the default minimum period needs it.  Returns dict(period, duration, objective, oversample, time_unit)."""
+        def _span():
+            if tmax is None:
+                raise ValueError("zero-size array to reduction operation maximum which has no identity")
+            return tmax - tmin
 
         duration = kwargs.pop("duration", [0.05, 0.10, 0.15, 0.20, 0.25, 0.33])
         duration = getattr(duration, "value", duration)
@@ -503,16 +524,15 @@ class BoxLeastSquaresPeriodogram(Periodogram):
         maximum_period = getattr(maximum_period, "value", maximum_period)
         if period is not None and ~np.all(np.isfinite(period)):
             raise ValueError("`period` parameter contains illegal nan or inf value(s)")
-        tval = np.asarray(lc.time.value, dtype=np.float64)
         if minimum_period is None:
             if period is None:
-                minimum_period = np.max([np.median(np.diff(tval)) * 4,
-                                         np.max(duration) + np.median(np.diff(tval))])
+                dt = median_dt() if callable(median_dt) else median_dt
+                minimum_period = np.max([dt * 4, np.max(duration) + dt])
             else:
                 minimum_period = np.min(period)
         if maximum_period is None:
             if period is None:
-                maximum_period = (np.max(tval) - np.min(tval)) / 3.0
+                maximum_period = _span() / 3.0
             else:
                 maximum_period = np.max(period)
 
@@ -521,7 +541,8 @@ class BoxLeastSquaresPeriodogram(Periodogram):
             raise ValueError("{} is not a valid value for `time_unit`".format(time_unit))
 
         frequency_factor = kwargs.pop("frequency_factor", 10)
-        df = frequency_factor * np.min(duration) / (np.max(tval) - np.min(tval)) ** 2
+        baseline = _span()
+        df = frequency_factor * np.min(duration) / baseline ** 2
         npoints = int(((1 / minimum_period) - (1 / maximum_period)) / df)
         if npoints > 1e7:
             raise ValueError("`period` contains {} points."
@@ -534,9 +555,10 @@ class BoxLeastSquaresPeriodogram(Periodogram):
                         "Consider setting `frequency_factor` to a higher value."
                         "".format(np.round(npoints, 4)))
         if period is None:
-            period = BoxLeastSquaresPeriodogram.autoperiod(tval, duration, minimum_period=minimum_period,
-                                                           maximum_period=maximum_period,
-                                                           frequency_factor=frequency_factor)
+            period = BoxLeastSquaresPeriodogram._autoperiod_baseline(baseline, duration,
+                                                                     minimum_period=minimum_period,
+                                                                     maximum_period=maximum_period,
+                                                                     frequency_factor=frequency_factor)
         period = np.atleast_1d(np.asarray(period, dtype=np.float64))
         duration = np.atleast_1d(np.asarray(duration, dtype=np.float64))
         objective = kwargs.pop("objective", None) or "likelihood"
@@ -551,8 +573,7 @@ class BoxLeastSquaresPeriodogram(Periodogram):
             raise TypeError("unexpected keyword arguments {}".format(sorted(kwargs)))
         if np.min(period) <= np.max(duration):
             raise ValueError("The maximum transit duration must be shorter than the minimum period")
-        return dict(lc=lc, time=tval, flux=np.asarray(lc.flux.value, dtype=np.float64), dy=dy, period=period,
-                    duration=duration, objective=objective, oversample=oversample, time_unit=time_unit)
+        return dict(period=period, duration=duration, objective=objective, oversample=oversample, time_unit=time_unit)
 
     @staticmethod
     def _finish(prep, res, b=0):
@@ -740,22 +761,26 @@ class BoxLeastSquaresPeriodogram(Periodogram):
         bad = np.flatnonzero(res["status"] == _lib.E_SINGULAR)
         if len(bad):
             raise np.linalg.LinAlgError("Singular matrix (periodogram {}: {!r})".format(bad[0], pgs[bad[0]]))
+        return [BoxLeastSquaresPeriodogram._k10_stats_dict(pg, times[b][0], per[b], tt[b], res, b)
+                for b, pg in enumerate(pgs)]
+
+    @staticmethod
+    def _k10_stats_dict(pg, tstart, period, transit_time, res, b):
+        """compute_stats' dict of light curve b of a host-mode engine.bls_stats result `res`; `pg` gives the flux unit
+        and time format (a periodogram or its light curve), `tstart` is its first cadence's time."""
         toff = res["transit_offsets"]
-        out = []
-        for b, pg in enumerate(pgs):
-            s = res["stats"][b]
-            tstart = times[b][0]
-            n = int(res["transit_n"][b])
-            if n > 0:
-                first = res["transit_first"][b]
-                transit_times = per[b] * np.arange(first, first + n) + (tt[b] - tstart)
-                counts = res["per_transit_count"][toff[b]:toff[b] + n].astype(int)
-                lls = res["per_transit_log_likelihood"][toff[b]:toff[b] + n].copy()
-            else:
-                transit_times, counts, lls = np.zeros(0), np.zeros(0, dtype=int), np.zeros(0)
-            out.append(pg._stats_dict(tstart, transit_times, counts, lls, (s[0], s[1]), (s[8], s[9]), (s[6], s[7]),
-                                      (s[2], s[3]), (s[4], s[5]), s[10], s[11]))
-        return out
+        s = res["stats"][b]
+        n = int(res["transit_n"][b])
+        if n > 0:
+            first = res["transit_first"][b]
+            transit_times = period * np.arange(first, first + n) + (transit_time - tstart)
+            counts = res["per_transit_count"][toff[b]:toff[b] + n].astype(int)
+            lls = res["per_transit_log_likelihood"][toff[b]:toff[b] + n].copy()
+        else:
+            transit_times, counts, lls = np.zeros(0), np.zeros(0, dtype=int), np.zeros(0)
+        return BoxLeastSquaresPeriodogram._stats_dict(pg, tstart, transit_times, counts, lls, (s[0], s[1]),
+                                                      (s[8], s[9]), (s[6], s[7]), (s[2], s[3]), (s[4], s[5]), s[10],
+                                                      s[11])
 
     @staticmethod
     def get_transit_mask_batch(periodograms, period=None, duration=None, transit_time=None):
