@@ -409,6 +409,58 @@ int lkb_nanmedian_std(const double* x, const int64_t* offsets, int B,
 int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_lo, const int32_t* win_hi, int W,
                      double corr_factor, double* background, int mem, void* stream);
 
+/* The same background for B periodograms on their own frequency grids (LightCurveCollection.to_seismology):
+ *   power        [bin_offsets[B]] fp32 or fp64 (p_dtype LKB_DTYPE_*), the periodograms back to back
+ *   bin_offsets  HOST CSR int64 [B+1]
+ *   win_lo/hi    HOST int32 [win_offsets[B]]: each periodogram's windows, relative to its first bin, ordered
+ *   win_offsets  HOST CSR int64 [B+1]
+ *   background   [bin_offsets[B]] fp64 out; snr: NULL or [bin_offsets[B]] fp64 out, power / background
+ *                (Periodogram.flatten's SNR spectrum).
+ * lkb_pg_logmedian is the shared-grid case of the same kernels.  Errors name the periodogram. */
+int lkb_pg_logmedian_ragged(const void* power, int p_dtype, const int64_t* bin_offsets, int B, const int32_t* win_lo,
+                            const int32_t* win_hi, const int64_t* win_offsets, double corr_factor, double* background,
+                            double* snr, int mem, void* stream);
+
+/* ---- gap filling (K15) ----------------------------------------------------------- */
+/* LightCurve.fill_gaps(method="gaussian_noise") for B light curves without cadence numbers; replaces the loop of
+ * lightcurve.py:1329-1427 (this repository's variant: insert prev += dt wherever t - prev > 1.2 dt, dt the median
+ * time step; flux_err by np.interp, flux = mean + std * z).  The host draws z between the two calls, in collection
+ * order, so that the inserted flux uses the deviates of np.random.normal's consecutive per-light-curve draws.
+ *
+ * lkb_fill_gaps_plan: for NaN-free light curves (t, flux [offsets[B]] fp64, offsets HOST CSR int64 [B+1]):
+ *   dt_out    [B] fp64: nanmedian(diff(t)) (K6; NaN for fewer than 2 cadences)
+ *   mean_out  [B] fp64: the mean flux (sum / n, NaN for n = 0)
+ *   n_ins_out [B] int64: the cadences the loop inserts
+ *   flags_out [B] int32: 1 = some step < 0 (the loop's in_original test then mis-assigns the flux), 2 = some step
+ *             > 0 (with dt <= 0 the loop never ends), 4 = a gap of more than 2^24 steps or a step dt too small to
+ *             advance the time; the caller refuses a light curve with flag 1, flags 2 with dt <= 0, or flag 4.
+ * lkb_fill_gaps: the filled light curves.
+ *   dt, mean, std  [B] fp64 (std: the CDPP in the flux unit, or nanstd, as the caller decides)
+ *   z              [out_offsets[B] - offsets[B]] fp64 standard normal deviates; light curve b's start at
+ *                  out_offsets[b] - offsets[b] (NULL when nothing is inserted)
+ *   out_offsets    HOST CSR int64 [B+1]: offsets[b+1] - offsets[b] + n_ins[b] cadences per light curve
+ *   t_out, flux_out, err_out [out_offsets[B]] fp64.  Times and flux_err are bitwise the loop's, flux is
+ *                  flux at original cadences and mean + std * z at inserted ones. */
+/* lkb_normalize_compact: lc.normalize().remove_nans() of B light curves (lightcurve.py:1216-1327), the first step of
+ * LightCurveCollection.to_seismology: flux / median[b] and flux_err / median[b], keeping the cadences whose normalized
+ * flux is not NaN, in order (a stable compaction).
+ *   t, flux, flux_err [offsets[B]] fp64; offsets HOST CSR int64 [B+1]; median [B] fp64 (lkb_nanmedian_std's)
+ *   out_offsets  HOST int64 [B+1] out: CSR of the kept cadences
+ *   bad_time     HOST int32 [B] out: 1 where a kept time is not finite
+ *   t_out, flux_out, err_out [offsets[B]] (allocate that many; out_offsets[B] are written)
+ *   ends         [2B] fp64 out: the first and last kept time (NaN without any)
+ * The call synchronises once, after counting, to build out_offsets.  The divisions are IEEE fp64, so they equal
+ * numpy's bit for bit. */
+int lkb_normalize_compact(const double* t, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+                          const double* median, int64_t* out_offsets, int32_t* bad_time, double* t_out,
+                          double* flux_out, double* err_out, double* ends, int mem, void* stream);
+int lkb_fill_gaps_plan(const double* t, const double* flux, const int64_t* offsets, int B, double* dt_out,
+                       double* mean_out, int64_t* n_ins_out, int32_t* flags_out, int mem, void* stream);
+int lkb_fill_gaps(const double* t, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+                  const double* dt, const double* mean, const double* std, const double* z,
+                  const int64_t* out_offsets, double* t_out, double* flux_out, double* err_out, int mem,
+                  void* stream);
+
 /* ---- periodogram autocorrelation (seismology ACF2D) ------------------------------ */
 /* K7: the autocorrelations behind the numax and deltanu estimators, for many windows of many series in one call.
  * Replaces seismology/utils.py:137-160 (autocorrelate), the per-numax loop of numax_estimators.py:170-182 and the

@@ -80,6 +80,12 @@ SIGNATURES = {
     "lkb_bin": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
                         c_int, c_vp]),
     "lkb_pg_logmedian": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_dbl, c_vp, c_int, c_vp]),
+    "lkb_pg_logmedian_ragged": (c_int, [c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_dbl, c_vp, c_vp, c_int, c_vp]),
+    "lkb_normalize_compact": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                      c_int, c_vp]),
+    "lkb_fill_gaps_plan": (c_int, [c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
+    "lkb_fill_gaps": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                              c_vp]),
     "lkb_acf_windows": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp]),
     "lkb_nccl_version": (c_int, []),
     "lkb_nccl_unique_id": (c_int, [c_vp]),

@@ -179,6 +179,133 @@ class LightCurveCollection(Collection):
                              for r, rs in enumerate(res["stats"])] for b in range(B)]
         return res
 
+    def fill_gaps(self, method="gaussian_noise"):
+        """Batched ``LightCurve.fill_gaps``: for the same ``np.random`` state, equal to
+        ``LightCurveCollection([lc.fill_gaps() for lc in collection])``, and it leaves the global RNG where that loop
+        leaves it.  The gap plan, the CDPP noise levels and the filled light curves come from one GPU call (K15, K6,
+        K4/K11/K12; ``engine.fill_gaps_device``); the host draws the normal deviates once, in collection order.
+
+        Times, flux_err and the flux of original cadences are bitwise the loop's.  Inserted flux is
+        ``nanmean(flux) + std * z`` with `std` the CDPP of ``lkb_cdpp`` (within about 1e-8 relative of the single
+        ``estimate_cdpp``) converted to the flux unit, or ``nanstd(flux)`` where ``estimate_cdpp().to(flux.unit)``
+        raises; for a light curve of two or more finite cadences that happens only when the flux unit cannot be
+        converted from ppm (for example electron/s).  The mean is a plain sum, so it may differ from numpy's pairwise
+        one in the last bits.  Float32 flux is worked in float64.
+
+        Raises ValueError, naming the light curve, for input the loop cannot handle: non-finite times, times that
+        decrease once the NaN fluxes are removed (the loop would then mis-assign the flux), a median time step <= 0
+        with some positive step (the loop would never end), and a gap of more than 2**24 median steps."""
+        from . import engine
+        from . import units as u
+        from .units import Quantity, Time
+        if method != "gaussian_noise":
+            raise NotImplementedError("No such method as {}".format(method))
+        if not self.data:
+            return LightCurveCollection([])
+        lcs = [lc.copy().remove_nans() for lc in self.data]
+        times = [np.asarray(lc.time.value, dtype=np.float64) for lc in lcs]
+        _check_finite_times(times)
+        fluxes = [np.asarray(lc.flux.value, dtype=np.float64) for lc in lcs]
+        errs = [np.asarray(lc.flux_err.value, dtype=np.float64) for lc in lcs]
+
+        def std(cdpp_ppm):
+            out = np.zeros(len(lcs))
+            for b, lc in enumerate(lcs):
+                if len(fluxes[b]) < 2:
+                    continue
+                try:
+                    out[b] = float(Quantity(cdpp_ppm[b], u.ppm).to(lc.flux.unit).value)
+                except Exception:                     # noqa: BLE001 - the single method's fallback
+                    out[b] = np.nanstd(fluxes[b])
+            return out
+
+        tt, yy, ee = engine.fill_gaps(times, fluxes, errs, std)
+        out = []
+        for b, lc in enumerate(lcs):
+            if len(times[b]) < 2:
+                out.append(lc)
+                continue
+            out.append(LightCurve(time=Time(tt[b], lc.time.format, lc.time.scale), flux=Quantity(yy[b], lc.flux.unit),
+                                  flux_err=Quantity(ee[b], lc.flux_err.unit), meta=self.data[b].meta))
+        return LightCurveCollection(out)
+
+    def to_seismology(self, **kwargs):
+        """Batched ``LightCurve.to_seismology``: a list of `Seismology` objects whose element b, for the same
+        ``np.random`` state, equals ``Seismology.from_lightcurve(lc_b, **kwargs)``, i.e. the SNR spectrum of
+        ``lc.normalize().remove_nans().fill_gaps().to_periodogram(**kwargs).flatten()``.  The whole chain runs in one
+        GPU call (``engine.seismology_spectra``): the raw light curves are uploaded once, normalized and cleared of
+        NaN fluxes on the device, and only arrays of one value per light curve and the final spectra come back.  The
+        next step is the batch estimators, e.g.::
+
+            seis = coll.to_seismology(normalization="psd")
+            numax = estimate_numax_acf2d_batch([s.periodogram for s in seis])
+
+        `kwargs` are those of ``to_periodogram("lombscargle")`` (normalization, minimum_frequency /
+        maximum_frequency, minimum_period / maximum_period, frequency / period, oversample_factor, nyquist_factor,
+        freq_unit, nterms, ls_method ...).  Each light curve has its own grid, so the power comes from the exact
+        direct sums (``lkb_ls_power``; ``lkb_ls_power_chi2`` for the multi-term methods "chi2", "fastchi2" and
+        "fastnifty_chi2"), which agree with the single call's kernels to the Lomb-Scargle parity tolerance.  The
+        normalization's median is the single ``normalize``'s K6 value and the division is IEEE fp64, so both are
+        bitwise the loop's; the inserted flux follows `LightCurveCollection.fill_gaps`.  Float32 flux is worked in
+        float64.
+
+        The `from_lightcurve` info message is logged once per call; ``normalize``'s warnings are raised for every
+        light curve that triggers them.  Errors: non-finite times among the kept cadences, then fill_gaps' refusals
+        (ValueError), then the loop's first periodogram error, of the same type, naming the light curve.  At most
+        65 535 light curves.  An empty collection returns []."""
+        from . import engine
+        from . import units as u
+        from .lightcurve import _normalize_warnings
+        from .periodogram import LombScarglePeriodogram as LS, SNRPeriodogram
+        from .seismology import Seismology
+        from .units import Quantity
+        if not self.data:
+            return []
+        logging.getLogger("lightkurve_b200.seismology").info(
+            "Building a Seismology object directly from a light curve "
+            "uses default periodogram parameters. For further tuneability, "
+            "create a periodogram object first, using `to_periodogram`.")
+        B = len(self.data)
+        preps = [None] * B
+
+        def warn(med, sd):
+            for b in range(B):
+                _normalize_warnings(float(med[b]), float(sd[b]))
+
+        def grid(b, median_dt, t_first, t_last, n):
+            empty = np.zeros(0)
+            span = (lambda: (np.median(np.diff(empty)), empty[-1], empty[0])) if n == 0 else \
+                (lambda: (np.float64(median_dt), np.float64(t_first), np.float64(t_last)))
+            try:
+                p = LS._grid(span, **dict(kwargs))
+                freq = np.asarray(p["frequency"].value, dtype=np.float64)
+                if len(freq) <= 1:
+                    raise ValueError("frequency and power must have a length greater than 1.")
+            except Exception as e:
+                raise _named(e, b) from e
+            preps[b] = p
+            scale = 2.0 / (n * p["oversample_factor"] * float(p["fs"].value)) if p["normalization"] == "psd" else None
+            return dict(frequency=np.asarray(p["frequency"].to(1 / u.day).value, dtype=np.float64), freq=freq,
+                        scale=scale, normalization=p["normalization"], nterms=p["nterms"],
+                        multiterm=p["ls_method"] in ("chi2", "fastchi2", "fastnifty_chi2"))
+
+        snr = engine.seismology_spectra([np.asarray(lc.time.value, dtype=np.float64) for lc in self.data],
+                                        [np.asarray(lc.flux.value, dtype=np.float64) for lc in self.data],
+                                        [np.asarray(lc.flux_err.value, dtype=np.float64) for lc in self.data], grid,
+                                        on_median=warn)
+        out = []
+        for b, lc in enumerate(self.data):
+            p = preps[b]
+            pu = u.dimensionless_unscaled if p["normalization"] == "amplitude" else \
+                u.dimensionless_unscaled ** 2 / p["freq_unit"]
+            unit = (Quantity(np.ones(1), pu) / Quantity(np.ones(1), pu)).unit
+            meta = dict(lc.copy(copy_data=False).meta)
+            meta["NORMALIZED"] = True
+            pg = SNRPeriodogram(p["frequency"], Quantity(snr[b], unit), nyquist=p["nyquist"],
+                                targetid=meta.get("TARGETID"), label=meta.get("LABEL"), meta=meta)
+            out.append(Seismology(pg))
+        return out
+
     def flatten(self, window_length=101, polyorder=2, return_trend=False, break_tolerance=5, niters=3, sigma=3,
                 mask=None):
         """Batched ``LightCurve.flatten``; `mask` is None or a list of per-LC boolean masks."""
@@ -363,6 +490,20 @@ class LightCurveCollection(Collection):
         new.flux_err = Quantity(np.concatenate([np.asarray(lc.flux_err.to(first.flux.unit).value) for lc in lcs]),
                                 first.flux.unit)
         return new
+
+
+def _check_finite_times(times):
+    for b, t in enumerate(times):
+        if not np.isfinite(t).all():
+            raise ValueError("light curve {} has non-finite times".format(b))
+
+
+def _named(e, b):
+    """`e` again, of the same type, with the light curve in front of its message."""
+    try:
+        return type(e)("light curve {}: {}".format(b, e))
+    except Exception:                                  # an exception type that needs other arguments
+        return e
 
 
 def _per_light_curve(value, B, name):

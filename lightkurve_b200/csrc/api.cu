@@ -227,6 +227,14 @@ int elasticnet(const double*, int, const double*, const uint8_t*, int, int64_t, 
                double*, double*, int32_t*, double*, uint8_t*, int, cudaStream_t);
 int nanmedian_std(const double*, const int64_t*, int, double*, double*, int, cudaStream_t);
 int pg_logmedian(const double*, int, int64_t, const int32_t*, const int32_t*, int, double, double*, int, cudaStream_t);
+int pg_logmedian_ragged(const void*, int, const int64_t*, int, const int32_t*, const int32_t*, const int64_t*, double,
+                        double*, double*, int, cudaStream_t);
+int normalize_compact(const double*, const double*, const double*, const int64_t*, int, const double*, int64_t*,
+                      int32_t*, double*, double*, double*, double*, int, cudaStream_t);
+int fill_gaps_plan(const double*, const double*, const int64_t*, int, double*, double*, int64_t*, int32_t*, int,
+                   cudaStream_t);
+int fill_gaps(const double*, const double*, const double*, const int64_t*, int, const double*, const double*,
+              const double*, const double*, const int64_t*, double*, double*, double*, int, cudaStream_t);
 int acf_windows(const double*, const int64_t*, int, const int64_t*, const int64_t*, const int64_t*, double*, double*,
                 int, cudaStream_t);
 int savgol_tables_host(int, int, double*, double*);
@@ -536,6 +544,37 @@ int lkb_pg_logmedian(const double* power, int B, int64_t F, const int32_t* win_l
                      double corr_factor, double* background, int mem, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   return pg_logmedian(power, B, F, win_lo, win_hi, W, corr_factor, background, mem, (cudaStream_t)stream);
+}
+
+int lkb_pg_logmedian_ragged(const void* power, int p_dtype, const int64_t* bin_offsets, int B, const int32_t* win_lo,
+                            const int32_t* win_hi, const int64_t* win_offsets, double corr_factor, double* background,
+                            double* snr, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return pg_logmedian_ragged(power, p_dtype, bin_offsets, B, win_lo, win_hi, win_offsets, corr_factor, background, snr,
+                             mem, (cudaStream_t)stream);
+}
+
+int lkb_normalize_compact(const double* t, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+                          const double* median, int64_t* out_offsets, int32_t* bad_time, double* t_out,
+                          double* flux_out, double* err_out, double* ends, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return normalize_compact(t, flux, flux_err, offsets, B, median, out_offsets, bad_time, t_out, flux_out, err_out, ends,
+                           mem, (cudaStream_t)stream);
+}
+
+int lkb_fill_gaps_plan(const double* t, const double* flux, const int64_t* offsets, int B, double* dt_out,
+                       double* mean_out, int64_t* n_ins_out, int32_t* flags_out, int mem, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return fill_gaps_plan(t, flux, offsets, B, dt_out, mean_out, n_ins_out, flags_out, mem, (cudaStream_t)stream);
+}
+
+int lkb_fill_gaps(const double* t, const double* flux, const double* flux_err, const int64_t* offsets, int B,
+                  const double* dt, const double* mean, const double* std, const double* z,
+                  const int64_t* out_offsets, double* t_out, double* flux_out, double* err_out, int mem,
+                  void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return fill_gaps(t, flux, flux_err, offsets, B, dt, mean, std, z, out_offsets, t_out, flux_out, err_out, mem,
+                   (cudaStream_t)stream);
 }
 
 int lkb_acf_windows(const double* x, const int64_t* x_offsets, int B, const int64_t* win_offsets,

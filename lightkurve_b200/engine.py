@@ -1166,6 +1166,239 @@ def pg_logmedian(frequency, power, filter_width):
     return out[0] if one else out
 
 
+def pg_logmedian_ragged(frequencies, power, filter_width, bin_offsets=None, snr=False):
+    """Periodogram.smooth(method="logmedian") of B periodograms on their own ascending frequency grids
+    (`frequencies`: list of host arrays).  `power`: list of host arrays (host mode), or the concatenated CUDA float32
+    / float64 tensor with its host int64 CSR `bin_offsets` (device mode, on the current torch stream).  Returns the
+    backgrounds and, with `snr`, also power / background (Periodogram.flatten), fp64: lists of arrays (host) or
+    concatenated tensors (device)."""
+    lib = L.load()
+    B = len(frequencies)
+    wins = [logmedian_windows(f, filter_width) for f in frequencies]
+    lo, woff = _csr([w[0] for w in wins], np.int32)
+    hi, _ = _csr([w[1] for w in wins], np.int32)
+    if _is_torch(power):
+        import torch
+        boff = _host_offsets(bin_offsets, "bin_offsets")
+        if len(boff) != B + 1 or any(boff[b + 1] - boff[b] != len(f) for b, f in enumerate(frequencies)):
+            raise ValueError("bin_offsets do not describe the frequency grids")
+        if power.dtype not in (torch.float32, torch.float64):
+            raise TypeError("power must be float32 or float64")
+        _device_csr(power, "power", power.dtype, int(boff[-1]))
+        n = max(int(boff[-1]), 1)
+        bkg = torch.empty(n, dtype=torch.float64, device=power.device)
+        out_snr = torch.empty(n, dtype=torch.float64, device=power.device) if snr else None
+        L.check(lib.lkb_pg_logmedian_ragged(L.ptr(power), L.DTYPE_F32 if power.dtype == torch.float32 else L.DTYPE_F64,
+                                            L.ptr(boff), B, L.ptr(lo), L.ptr(hi), L.ptr(woff), (8.0 / 9.0) ** 3,
+                                            L.ptr(bkg), L.ptr(out_snr), L.MEM_DEVICE, _stream_ptr()))
+        nb = int(boff[-1])
+        return (bkg[:nb], out_snr[:nb]) if snr else bkg[:nb]
+    p, boff = _csr(power)
+    if len(boff) != B + 1 or any(boff[b + 1] - boff[b] != len(f) for b, f in enumerate(frequencies)):
+        raise ValueError("power and frequency lengths differ")
+    bkg = np.empty(max(len(p), 1))
+    out_snr = np.empty(max(len(p), 1)) if snr else None
+    L.check(lib.lkb_pg_logmedian_ragged(L.ptr(p), L.DTYPE_F64, L.ptr(boff), B, L.ptr(lo), L.ptr(hi), L.ptr(woff),
+                                        (8.0 / 9.0) ** 3, L.ptr(bkg), L.ptr(out_snr), L.MEM_HOST, None))
+    sp = lambda x: [x[boff[b]:boff[b + 1]] for b in range(B)]
+    return (sp(bkg), sp(out_snr)) if snr else sp(bkg)
+
+
+# --------------------------------------------------------------------------------------
+# gap filling and the seismology spectra (K15)
+# --------------------------------------------------------------------------------------
+GAP_DECREASING, GAP_POSITIVE, GAP_TOO_LONG = 1, 2, 4
+
+
+def _gap_reject(b, flags, dt):
+    """The ValueError for light curve b that fill_gaps refuses (the loop would mis-assign or never end), or None."""
+    if flags & GAP_DECREASING:
+        return ValueError("light curve %d: its times decrease; fill_gaps needs them in order" % b)
+    if flags & GAP_POSITIVE and not dt > 0:
+        return ValueError("light curve %d: the median time step is %r while some step is positive; the gap "
+                          "filling loop would never end" % (b, float(dt)))
+    if flags & GAP_TOO_LONG:
+        return ValueError("light curve %d: a gap spans more than 2**24 median time steps, or the median step is too "
+                          "small to advance the time" % b)
+    return None
+
+
+def fill_gaps_device(d_t, d_y, d_e, offsets, std):
+    """K15 (+ K6 for the median step): LightCurve.fill_gaps(method="gaussian_noise") of the NaN-free light curves in
+    the concatenated CUDA float64 tensors `d_t` (finite times), `d_y`, `d_e` with the host int64 CSR `offsets`.
+    `std(plan)` returns the host [B] noise levels, given plan = dict(dt, mean, n_ins, flags) (host arrays; called
+    after the plan's one synchronisation).  Refused light curves raise ValueError naming the first; then the normal
+    deviates come from ONE np.random.standard_normal(sum of n_ins) draw, which equals the loop's consecutive
+    np.random.normal(mean, std, n_ins[b]) draws.  Returns (t, flux, flux_err, out_offsets, plan), CUDA tensors and
+    host arrays."""
+    import torch
+    lib = L.load()
+    off = _host_offsets(offsets, "offsets")
+    B, n = len(off) - 1, int(off[-1])
+    for name, x in (("t", d_t), ("flux", d_y), ("flux_err", d_e)):
+        _device_csr(x, name, torch.float64)
+        if x.numel() < max(n, 1):
+            raise ValueError("device mode: %s has fewer values than the offsets describe" % name)
+    dev = d_t.device
+    dt, mean = torch.empty(B, dtype=torch.float64, device=dev), torch.empty(B, dtype=torch.float64, device=dev)
+    n_ins = torch.empty(B, dtype=torch.int64, device=dev)
+    flags = torch.empty(B, dtype=torch.int32, device=dev)
+    L.check(lib.lkb_fill_gaps_plan(L.ptr(d_t), L.ptr(d_y), L.ptr(off), B, L.ptr(dt), L.ptr(mean), L.ptr(n_ins),
+                                   L.ptr(flags), L.MEM_DEVICE, _stream_ptr()))
+    plan = dict(dt=dt.cpu().numpy(), mean=mean.cpu().numpy(), n_ins=n_ins.cpu().numpy(), flags=flags.cpu().numpy())
+    for b in range(B):
+        e = _gap_reject(b, int(plan["flags"][b]), plan["dt"][b])
+        if e is not None:
+            raise e
+    s = np.ascontiguousarray(std(plan), dtype=np.float64)
+    noff = off.copy()
+    noff[1:] += np.cumsum(plan["n_ins"])
+    nz = int(noff[-1] - off[-1])
+    z = torch.from_numpy(np.ascontiguousarray(np.random.standard_normal(nz))).to(dev) if nz else None
+    d_s = torch.from_numpy(s).to(dev)
+    nn = max(int(noff[-1]), 1)
+    t2, y2, e2 = (torch.empty(nn, dtype=torch.float64, device=dev) for _ in range(3))
+    L.check(lib.lkb_fill_gaps(L.ptr(d_t), L.ptr(d_y), L.ptr(d_e), L.ptr(off), B, L.ptr(dt), L.ptr(mean), L.ptr(d_s),
+                              L.ptr(z), L.ptr(noff), L.ptr(t2), L.ptr(y2), L.ptr(e2), L.MEM_DEVICE, _stream_ptr()))
+    plan["std"] = s
+    return t2, y2, e2, noff, plan
+
+
+def fill_gaps(times, fluxes, flux_errs, std):
+    """`fill_gaps_device` for lists of host float64 arrays (NaN-free flux, finite times), uploaded once.  `std(cdpp)`
+    gets the [B] CDPP in ppm (lkb_cdpp with estimate_cdpp's defaults, on the device copies) and returns the [B]
+    noise levels.  Returns the filled times, fluxes and flux errors as lists of host arrays."""
+    import torch
+    t_h, off = _csr(times)
+    B, n = len(times), int(off[-1])
+    dev = torch.device("cuda", torch.cuda.current_device())
+    d_t, d_y, d_e = (torch.from_numpy(_csr(a)[0] if n else np.zeros(1)).to(dev) for a in (times, fluxes, flux_errs))
+
+    def level(plan):
+        return std(cdpp(d_t[:n], d_y[:n], 13, offsets=off).cpu().numpy()[:, 0] if n else np.zeros(B))
+
+    t2, y2, e2, noff, _ = fill_gaps_device(d_t, d_y, d_e, off, level)
+    tt, yy, ee = (x.cpu().numpy() for x in (t2, y2, e2))
+    sl = [slice(noff[b], noff[b + 1]) for b in range(B)]
+    return [tt[x].copy() for x in sl], [yy[x].copy() for x in sl], [ee[x].copy() for x in sl]
+
+
+SEISMOLOGY_MAX_B = 65535
+
+
+def seismology_spectra(times, fluxes, flux_errs, grid, on_median=None, filter_width=0.01):
+    """K6 + normalize/compact + K15 + K4/K11/K12 + K1 (or K1n) + the ragged log-median: the SNR spectra of
+    ``lc.normalize().remove_nans().fill_gaps().to_periodogram(**kwargs).flatten()`` for every light curve.
+    `times`, `fluxes`, `flux_errs`: lists of host float64 arrays, the raw light curves, uploaded once.  On the device:
+    the K6 nanmedian and nanstd of the flux (`on_median(median, std)` gets them on the host, for normalize's
+    warnings), flux and flux_err divided by the median with the NaN fluxes dropped (lkb_normalize_compact), K15 with
+    the CDPP (lkb_cdpp, estimate_cdpp's defaults, converted from ppm to the dimensionless flux) as the noise level,
+    K15's plan again for the median step of the filled times, the periodograms and their log-median SNR.
+    `grid(b, median_dt, t_first, t_last, n)` returns dict(frequency (1/day), freq (the grid in its own unit),
+    scale (psd scale or None), normalization, nterms, multiterm) or raises as the loop would.  Kept times must be
+    finite (ValueError naming the light curve); fill_gaps' refusals come next, then the first grid error.
+    Returns the list of SNR arrays (in each grid's order)."""
+    import torch
+    lib = L.load()
+    from . import units as u
+    B = len(times)
+    if not 0 < B <= SEISMOLOGY_MAX_B:
+        raise ValueError("seismology_spectra needs 1 .. %d light curves, got %d" % (SEISMOLOGY_MAX_B, B))
+    t_h, off = _csr(times)
+    y_h, yoff = _csr(fluxes)
+    e_h, eoff = _csr(flux_errs)
+    if not (np.array_equal(off, yoff) and np.array_equal(off, eoff)):
+        raise ValueError("time, flux and flux_err lengths differ")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    f64 = dict(dtype=torch.float64, device=dev)
+
+    def up(a):
+        x = torch.empty(max(len(a), 1), **f64)
+        x[:len(a)].copy_(torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)))
+        return x
+
+    n0 = int(off[-1])
+    d_t, d_y, d_e = up(t_h), up(y_h), up(e_h)
+    # 1. normalize().remove_nans(): the K6 median (only [B] values come back), the division and the compaction
+    med, sd = torch.empty(B, **f64), torch.empty(B, **f64)
+    L.check(lib.lkb_nanmedian_std(L.ptr(d_y), L.ptr(off), B, L.ptr(med), L.ptr(sd), L.MEM_DEVICE, _stream_ptr()))
+    if on_median is not None:
+        on_median(med.cpu().numpy(), sd.cpu().numpy())
+    noff = np.zeros(B + 1, np.int64)
+    bad = np.zeros(B, np.int32)
+    t1, y1, e1 = (torch.empty(max(n0, 1), **f64) for _ in range(3))
+    ends = torch.empty(2 * B, **f64)
+    L.check(lib.lkb_normalize_compact(L.ptr(d_t), L.ptr(d_y), L.ptr(d_e), L.ptr(off), B, L.ptr(med), L.ptr(noff),
+                                      L.ptr(bad), L.ptr(t1), L.ptr(y1), L.ptr(e1), L.ptr(ends), L.MEM_DEVICE,
+                                      _stream_ptr()))
+    del d_t, d_y, d_e
+    for b in np.flatnonzero(bad):
+        raise ValueError("light curve %d has non-finite times" % b)
+    ends_h = ends.cpu().numpy().reshape(B, 2)
+    n = int(noff[-1])
+    ppm = float(u.Quantity(1.0, u.ppm).to(u.dimensionless_unscaled).value)
+
+    def std(plan):
+        if n == 0:
+            return np.zeros(B)
+        return cdpp(t1[:n], y1[:n], 13, offsets=noff).cpu().numpy()[:, 0] * ppm
+
+    # 2. fill_gaps
+    t2, y2, e2, foff, plan = fill_gaps_device(t1, y1, e1, noff, std)
+    del t1, y1, e1
+    if np.any((plan["n_ins"] > 0) & ~np.isfinite(plan["mean"] + plan["std"])):
+        # NaN inserted flux: the periodogram's own remove_nans drops those cadences
+        tt, yy, ee = (x.cpu().numpy()[:int(foff[-1])] for x in (t2, y2, e2))
+        keep = ~np.isnan(yy)
+        lens = np.array([int(keep[foff[b]:foff[b + 1]].sum()) for b in range(B)], dtype=np.int64)
+        foff = np.zeros(B + 1, np.int64)
+        np.cumsum(lens, out=foff[1:])
+        t2, y2, e2 = up(tt[keep]), up(yy[keep]), up(ee[keep])
+    # 3. the grids: median step of the filled times (K15's plan entry runs K6 on the steps), first and last time, N
+    N = np.diff(foff)
+    md = torch.empty(B, **f64)
+    scratch = [torch.empty(B, **f64), torch.empty(B, dtype=torch.int64, device=dev),
+               torch.empty(B, dtype=torch.int32, device=dev)]
+    L.check(lib.lkb_fill_gaps_plan(L.ptr(t2), L.ptr(y2), L.ptr(foff), B, L.ptr(md), L.ptr(scratch[0]),
+                                   L.ptr(scratch[1]), L.ptr(scratch[2]), L.MEM_DEVICE, _stream_ptr()))
+    md_h = md.cpu().numpy()
+    grids = [grid(b, md_h[b], ends_h[b, 0] if N[b] else None, ends_h[b, 1] if N[b] else None, int(N[b]))
+             for b in range(B)]
+    # 4. the periodograms, on grids in ascending frequency (Periodogram.smooth sorts a descending one)
+    orders = [None if len(g["freq"]) < 2 or np.all(np.diff(g["freq"]) >= 0) else np.argsort(g["freq"], kind="stable")
+              for g in grids]
+    sorted_f = [g["frequency"] if o is None else g["frequency"][o] for g, o in zip(grids, orders)]
+    freq_h, pofs = _csr(sorted_f)
+    g0 = grids[0]
+    scale = None
+    if g0["scale"] is not None:
+        scale = torch.from_numpy(np.ascontiguousarray([g["scale"] for g in grids], dtype=np.float64)).to(dev)
+    d_f = up(freq_h)
+    F = int(pofs[-1])
+    power = torch.empty(max(F, 1), dtype=torch.float32, device=dev)
+    if g0["multiterm"]:
+        L.check(lib.lkb_ls_power_chi2_ex(L.ptr(t2), L.ptr(y2), L.DTYPE_F64, L.ptr(foff), B, L.ptr(d_f), L.ptr(pofs), F,
+                                         int(g0["nterms"]), _NORMS[g0["normalization"]], L.ptr(scale), L.ptr(power),
+                                         None, L.MEM_DEVICE, _stream_ptr(), L.LS_ALGO_SIMT))
+    else:
+        L.check(lib.lkb_ls_power_ex(L.ptr(t2), L.ptr(y2), L.DTYPE_F64, L.ptr(foff), B, L.ptr(d_f), L.ptr(pofs), F,
+                                    _NORMS[g0["normalization"]], L.ptr(scale), L.ptr(power), L.MEM_DEVICE,
+                                    _stream_ptr(), L.LS_ALGO_AUTO))
+    # 5. the log-median background and the SNR
+    _, snr = pg_logmedian_ragged([g["freq"] if o is None else g["freq"][o] for g, o in zip(grids, orders)],
+                                 power[:F] if F else power, filter_width, bin_offsets=pofs, snr=True)
+    snr_h = snr.cpu().numpy()
+    out = []
+    for b, o in enumerate(orders):
+        x = snr_h[pofs[b]:pofs[b + 1]]
+        if o is not None:
+            inv = np.empty_like(o)
+            inv[o] = np.arange(len(o))
+            x = x[inv]
+        out.append(x.copy())
+    return out
+
+
 # bytes of series + outputs staged on the device by one lkb_acf_windows call; larger batches are split by series
 ACF_STAGE_BYTES = 2 << 30
 

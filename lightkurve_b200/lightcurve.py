@@ -125,6 +125,27 @@ def _bin_edges(n, t_first, t_last, time_bin_size, time_bin_start, time_bin_end, 
     return "time", starts, starts + size
 
 
+def _normalize_warnings(median_flux, std_flux):
+    """The LightkurveWarnings of `LightCurve.normalize` for a flux of this nanmedian and nanstd."""
+    if (median_flux == 0) or (np.isfinite(std_flux) and (np.abs(median_flux) < 0.5 * std_flux)):
+        warnings.warn(
+            "The light curve appears to be zero-centered "
+            "(median={:.2e} +/- {:.2e}); `normalize()` will divide "
+            "the light curve by a value close to zero, which is "
+            "probably not what you want."
+            "".format(median_flux, std_flux),
+            LightkurveWarning,
+        )
+    if median_flux < 0:
+        warnings.warn(
+            "The light curve has a negative median flux ({:.2e});"
+            " `normalize()` will therefore divide by a negative "
+            "number and invert the light curve, which is probably"
+            "not what you want".format(median_flux),
+            LightkurveWarning,
+        )
+
+
 class LightCurve:
     """Time series of flux values (subset of lightkurve.LightCurve).
 
@@ -303,23 +324,7 @@ class LightCurve:
         from . import engine
         med, sd = engine.nanmedian_std([np.asarray(self.flux.value, dtype=np.float64)])
         median_flux, std_flux = float(med[0]), float(sd[0])
-        if (median_flux == 0) or (np.isfinite(std_flux) and (np.abs(median_flux) < 0.5 * std_flux)):
-            warnings.warn(
-                "The light curve appears to be zero-centered "
-                "(median={:.2e} +/- {:.2e}); `normalize()` will divide "
-                "the light curve by a value close to zero, which is "
-                "probably not what you want."
-                "".format(median_flux, std_flux),
-                LightkurveWarning,
-            )
-        if median_flux < 0:
-            warnings.warn(
-                "The light curve has a negative median flux ({:.2e});"
-                " `normalize()` will therefore divide by a negative "
-                "number and invert the light curve, which is probably"
-                "not what you want".format(median_flux),
-                LightkurveWarning,
-            )
+        _normalize_warnings(median_flux, std_flux)
         lc = self.copy()
         with np.errstate(divide="ignore", invalid="ignore"):
             lc.flux = Quantity(self.flux.value / median_flux, u.dimensionless_unscaled)

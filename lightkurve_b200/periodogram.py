@@ -234,6 +234,23 @@ class LombScarglePeriodogram(Periodogram):
             lc = lc.remove_nans()
             log.debug("Lightcurve contains NaN values."
                       "These are removed before creating the periodogram.")
+        time = lc.time.copy()
+        tval = np.asarray(time.value, dtype=np.float64)
+        out = LombScarglePeriodogram._grid(lambda: (np.median(np.diff(tval)), tval[0], tval[-1]),
+                                           minimum_frequency, maximum_frequency, minimum_period, maximum_period,
+                                           frequency, period, nterms, nyquist_factor, oversample_factor, freq_unit,
+                                           normalization, ls_method, **kwargs)
+        out.update(lc=lc, time=tval)
+        return out
+
+    @staticmethod
+    def _grid(span, minimum_frequency=None, maximum_frequency=None, minimum_period=None, maximum_period=None,
+              frequency=None, period=None, nterms=1, nyquist_factor=1, oversample_factor=None, freq_unit=None,
+              normalization="amplitude", ls_method="fast", **kwargs):
+        """The grid part of `_prepare`, for a light curve described by `span()` = (np.median(np.diff(t)), t[0], t[-1])
+        (called where `_prepare` reads the times, so that errors come in the same order).  Returns the dict of
+        `_prepare` without "lc" and "time"; its warnings and errors are `_prepare`'s."""
+        normalization = validate_method(normalization, ["psd", "amplitude"])
         if freq_unit is None:
             freq_unit = _PER_DAY if normalization == "amplitude" else u.microhertz
         freq_unit = u._as_unit(freq_unit)
@@ -267,10 +284,9 @@ class LombScarglePeriodogram(Periodogram):
             raise ValueError("You have input keyword arguments for both frequency and period. "
                              "Please only use one.")
 
-        time = lc.time.copy()
-        tval = np.asarray(time.value, dtype=np.float64)
-        nyquist = Quantity(0.5 * (1.0 / (np.median(np.diff(tval)))), _PER_DAY)
-        fs = Quantity((1.0 / (tval[-1] - tval[0])) / oversample_factor, _PER_DAY)
+        median_dt, t_first, t_last = span()
+        nyquist = Quantity(0.5 * (1.0 / median_dt), _PER_DAY)
+        fs = Quantity((1.0 / (t_last - t_first)) / oversample_factor, _PER_DAY)
         nyquist = nyquist.to(freq_unit)
         fs = fs.to(freq_unit)
 
@@ -339,7 +355,7 @@ class LombScarglePeriodogram(Periodogram):
         if ls_method not in ("fast", "slow", "auto", "cython", "scipy", "chi2", "fastchi2", "fastnifty",
                              "fastnifty_chi2"):
             raise ValueError("unknown ls_method '{}'".format(ls_method))
-        return dict(lc=lc, time=tval, frequency=frequency, freq_unit=freq_unit, fs=fs, nyquist=nyquist,
+        return dict(frequency=frequency, freq_unit=freq_unit, fs=fs, nyquist=nyquist,
                     oversample_factor=oversample_factor, normalization=normalization, ls_method=ls_method,
                     nterms=nterms, default_view=default_view)
 
